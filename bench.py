@@ -2,7 +2,7 @@
 """bench.py — headline benchmark of the hot path (BASELINE.json configs[1]):
 threshold -> seeded flood-fill region grow -> marching cubes on a 512^3 int16 CT phantom.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0).
 
@@ -20,11 +20,13 @@ One JSON line on stdout (rank 0).
             reference on the same 512^3 volume (reached-voxel count, mask equality, V, T, the
             triangle array and the vertices); N > 1 against a single-GPU run of the whole
             gathered volume on rank 0 (count, V, T, order-independent checksums of both arrays).
-`roofline`  the dominant stage against the measured HBM peak.
+`roofline`  the dominant stage against the HBM bandwidth of the H100 SXM data sheet.
 `cpu_baseline` / `--impl reference`  the CPU restatement of the reference path timed on this
             box's host cores on the SAME 512^3 volume (full, not a slab).
 `extra`     (N = 1) driver-visible secondary results: 1024^3 threshold / MaxIP x3 / MIDA with
             their roofline fractions, 512^3 watershed times + agreement with the CPU checker.
+`--dump-outputs DIR`  (one GPU only) after the timed steps, writes what the last timed step
+            computed as DIR/<name>.npy (float32 / float64, < 64 MB in all; see dump_outputs).
 """
 from __future__ import annotations
 
@@ -56,11 +58,9 @@ def workload_desc(n, world):
             f"iso 127 on the grown mask")
 
 
-def measured_peak():
-    try:
-        return float(json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"]), "measured"
-    except Exception:
-        return 6650.0, "fallback"
+def hbm_peak():
+    """HBM3 bandwidth of the H100 SXM data sheet (GB/s): a bound, not a measured rate."""
+    return 3350.0, "H100 SXM data sheet"
 
 
 def global_seed(n, world):
@@ -132,8 +132,8 @@ class ClockSampler:
     """SM clock and throttle reasons of one GPU, sampled DURING the warm-up and the timed region.
 
     In-process NVML (the library behind nvidia-smi) on a background thread: an `nvidia-smi -lms`
-    child stalls this process's host-synchronous CUDA calls for milliseconds at every poll (measured:
-    +0.3 .. +0.6 ms per step on a 1.3 ms step), which a 13 ms timed region cannot absorb. The
+    child stalls this process's host-synchronous CUDA calls for milliseconds at every poll, which a
+    timed region of a few milliseconds cannot absorb. The
     subprocess remains as the fallback when pynvml is missing."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -266,6 +266,37 @@ def checksums(verts, tris):
     tsum = int(tris.to(torch.int64).sum().item()) if tris.numel() else 0
     vsum = int(verts.contiguous().view(torch.int32).to(torch.int64).sum().item()) if verts.numel() else 0
     return tsum, vsum
+
+
+def dump_outputs(dirpath, mask, grown, verts, tris):
+    """What one step hands its caller, as .npy files comparable between two builds: the threshold
+    mask and the grown mask (the same fixed, seeded sample of 2^20 voxels of each, plus per-plane
+    counts over the whole volume), the mesh's vertex and triangle counts and its vertices (float32)
+    and triangles (float64), whole when they fit 16 / 24 MB, else a seeded sample of rows.
+    Under 64 MB in all."""
+    import torch
+    dirpath.mkdir(parents=True, exist_ok=True)
+    rng = np.random.default_rng(0)
+    vox = np.unique(rng.integers(0, mask.numel(), 1 << 20))
+    ti = torch.from_numpy(vox).to(mask.device)
+    out = {"voxel_index": vox.astype(np.float64),
+           "threshold_mask_sample": mask.reshape(-1)[ti].cpu().numpy().astype(np.float32),
+           "grown_mask_sample": grown.reshape(-1)[ti].cpu().numpy().astype(np.float32),
+           "threshold_plane_counts": (mask == 255).sum(dim=(1, 2)).cpu().numpy().astype(np.float64),
+           "grown_plane_counts": (grown == FILL).sum(dim=(1, 2)).cpu().numpy().astype(np.float64),
+           "mesh_counts": np.array([verts.shape[0], tris.shape[0]], np.float64)}
+
+    def rows(t, limit_bytes, dtype):
+        a = t.cpu().numpy()
+        keep = limit_bytes // (a.shape[1] * np.dtype(dtype).itemsize)
+        if len(a) > keep:
+            a = a[np.sort(np.random.default_rng(1).choice(len(a), keep, replace=False))]
+        return a.astype(dtype)
+
+    out["vertices"] = rows(verts, 16 << 20, np.float32)
+    out["triangles"] = rows(tris, 24 << 20, np.float64)
+    for name, a in out.items():
+        np.save(dirpath / f"{name}.npy", a)
 
 
 # ------------------------------------------------------------------ secondary results (N = 1)
@@ -451,10 +482,12 @@ def run_gpu(args):
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.dump_outputs and world > 1:
+        raise SystemExit("--dump-outputs writes the outputs of a one-GPU step; run it with --gpus 1")
     dev.require_cuda()
     torch.cuda.set_device(local)
     numa = bind_to_gpu_numa(local)
-    torch.set_num_threads(16)   # host memset of the out mask: 128 OpenMP threads make it erratic (0.3 .. 25 ms)
+    torch.set_num_threads(16)   # host memset of the out mask: one OpenMP thread per core of a large host makes it erratic
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     lib = _lib.load()
@@ -617,6 +650,8 @@ def run_gpu(args):
         barrier()
         if head:
             launches = int(lib.b2v_launch_count())
+            if args.dump_outputs:
+                dump_outputs(Path(args.dump_outputs), d_mask, shard.interior(d_out), v, f)
         total_ms = max_over_ranks(e0.elapsed_time(e1))
         if sampler:
             clocks = sampler.stop()
@@ -693,7 +728,7 @@ def run_gpu(args):
         barrier()
 
     # ---- e2e leg: reference-shaped numpy API on pinned host buffers
-    e2e_steps = max(1, min(args.steps, 5))
+    e2e_steps = args.steps
     v, f = step_e2e()
     v, f = step_e2e()   # results stay bound across calls, as in the timed loop: the pinned result
     v, f = step_e2e()   # pool reaches its steady state (two sets of blocks in flight)
@@ -731,21 +766,13 @@ def run_gpu(args):
         if world > 1:
             dist.destroy_process_group()
         return
-    peak, peak_kind = measured_peak()
+    peak, peak_kind = hbm_peak()
     # dominant stage and its roofline (algorithmic bytes: SURVEY.md 8d / DESIGN.md)
     alg = {"threshold": 3.0 * N, "floodfill": 4.0 * N,
            "marching_cubes": 1.0 * N + (12.0 * info["V"] + 12.0 * info["T"]) / world}
     names = list(alg)
     dom = int(np.argmax(stage_ms))
     achieved = alg[names[dom]] / (stage_ms[dom] * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    for cand in ("r02_traffic.json", "r01_traffic.json"):
-        try:   # DRAM bytes per launch of that stage from the committed ncu capture (profiles/)
-            traffic = json.load(open(ROOT / "profiles" / cand))["stages"][names[dom]]["traffic"]
-            traffic_src = f"profiles/{cand}"
-            break
-        except Exception:
-            pass
     seeding = {}
     for name, t in timed.items():
         seeding[name] = {"ms_per_step": round(t["ms_per_step"], 4),
@@ -758,7 +785,7 @@ def run_gpu(args):
         "scaling": "weak", "vs_baseline": None, "dtype": "int16", "data": "synthetic",
         "config": {"workload": workload_desc(n, world),
                    "volume": f"{n * world}x{n}x{n} (Z-sharded, one halo plane per inner side)",
-                   "shard": f"{n}^3 voxels per GPU", "l2": "inputs (256 MiB int16 + 128 MiB uint8) exceed the 126 MB L2",
+                   "shard": f"{n}^3 voxels per GPU", "l2": "inputs (256 MiB int16 + 128 MiB uint8) exceed the 50 MB L2",
                    "host": numa, "flood_rounds": info["rounds"], "vertices": info["V"], "triangles": info["T"],
                    "stage_ms": {k: round(float(m), 4) for k, m in zip(names, stage_ms)},
                    "seeding": seeding, "exchange": (link.describe() if link is not None else
@@ -774,8 +801,7 @@ def run_gpu(args):
                        "dist.* sharded pipeline fed from / drained to pinned host buffers (image uploaded once per step)",
                 "session": sess},
         "roofline": {"bound": "hbm", "kernel": names[dom], "achieved": round(achieved, 1), "peak": peak,
-                     "peak_kind": peak_kind, "unit": "GB/s", "frac": round(achieved / peak, 4), "traffic": traffic,
-                     "traffic_source": traffic_src,
+                     "peak_kind": peak_kind, "unit": "GB/s", "frac": round(achieved / peak, 4),
                      "note": "stage-level: algorithmic bytes of the dominant stage / its CUDA-event time; the flood's "
                              "rounds are L2/latency-bound, see DESIGN.md",
                      "per_stage_GBs": {k: round(alg[k] / (m * 1e-3) / 1e9, 1) for k, m in zip(names, stage_ms)},
@@ -854,7 +880,12 @@ def main():
     ap.add_argument("--cpu-slices", type=int, default=0, help="reference arm: time a slab of this many slices instead "
                                                               "of the full volume (0 = full volume, the default)")
     ap.add_argument("--no-extra", action="store_true", help="skip the secondary 1024^3 / watershed measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="one GPU: write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU path, not to --impl reference")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-"""invesalius3_b200 — Blackwell-native (sm_100a) volumetric compute core for InVesalius 3.
+"""invesalius3_b200 — H100-native (sm_90a) volumetric compute core for InVesalius 3.
 
 Drop-in replacement for the per-voxel hot path (threshold, MIP/MIDA, flood fill, watershed,
 marching cubes) behind the reference's numpy-in/numpy-out signatures:

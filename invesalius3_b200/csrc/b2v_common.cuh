@@ -1,4 +1,4 @@
-// b2v — Blackwell-native volumetric compute core (sm_100a).
+// b2v — volumetric compute core for the H100 (sm_90a).
 // Shared device/host helpers for every translation unit of libb2v.so.
 #pragma once
 #include <cuda_runtime.h>
@@ -7,7 +7,7 @@
 
 #include "../../include/b2v.h"
 
-#define B2V_SM_COUNT_FALLBACK 148
+#define B2V_SM_COUNT_FALLBACK 132
 
 // ---- error plumbing -------------------------------------------------------
 void b2v_set_error(const char* fmt, ...);

@@ -10,7 +10,7 @@
 // the structuring-element offsets. We compute that set in three steps:
 //   1. build   (HBM-bound, 3 B/voxel): one pass over data (+out) packs `passable` into a
 //              bit volume, 32 voxels per word along x. 512^3 voxels -> 16 MiB, i.e. the
-//              whole working set of step 2 lives in the B200's 126 MB L2.
+//              whole working set of step 2 lives in the H100's 50 MB L2.
 //   2. flood   (L2 / shared-memory latency-bound): tiles of the two bit volumes are pulled
 //              into shared memory, swept once along x (run fill by the carry trick), y and
 //              z, written back; the tiles that can gain from a grown tile are activated for
@@ -1187,7 +1187,7 @@ int run_persistent(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_
   int grid = per_sm * b2v_sm_count();        // every co-resident slot: one tile per block per round
   if (knobs().grid > 0 && knobs().grid < grid) grid = knobs().grid;   // tuning knob
   if (grid > ntiles) grid = (int)ntiles;
-  // a block keeps at most kMaxMine tiles of a round in shared memory (5 G voxels at 148 blocks and 16^3-word tiles)
+  // a block keeps at most kMaxMine tiles of a round in shared memory (4.4 G voxels at 132 blocks and 16^3-word tiles)
   if ((int64_t)grid * kMaxMine < ntiles) {
     B2V_REQUIRE(!peer, B2V_ERR_ARG, "floodfill: shard too large for the fused peer exchange (%d tiles)", ntiles);
     return run_rounds(b, w, sb, s, r0, rounds_out);

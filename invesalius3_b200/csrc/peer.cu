@@ -61,7 +61,7 @@ int peer_make_set(int rank, int world, const void* const* mailboxes_host, int64_
   out->world = world;
   out->epoch = epoch;
   out->pc = plane_bytes;
-  // ~4 s of SM clocks. The clock-rate attribute is one of the slow driver queries (~0.5 ms):
+  // ~4 s of SM clocks. The clock-rate attribute is one of the slow driver queries:
   // asked once per process, not per call.
   static long long cached_timeout = 0;
   if (cached_timeout == 0) {

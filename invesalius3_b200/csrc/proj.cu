@@ -449,10 +449,10 @@ __global__ void __launch_bounds__(kRays) k_rays_alongx_tma(const int16_t* __rest
   rays_alongx_tma<U, Op>(vol, d, op, true, out, status);
 }
 
-// Measured at 1024^3 (tools/mida_axis2.py, profiles/README.md): MIDA full rays 1.83 ms (TMA rows) vs
-// 1.68 ms (lane loads), LMIP 0.088 vs 0.052 ms — 128-byte bulk copies per thread are too small for the
-// copy engine to beat 32-bit lane loads here, and the rays are bound by the recurrence, not by the
-// loads. The lane-load kernels stay the default; b2v_proj_set_tma(1) (or B2V_TMA=1) selects this path.
+// Measured at 1024^3, rays along x (tools/mida_axis2.py, two alternating runs on one H100 80GB HBM3 at
+// a 400 W power limit): MIDA full rays 2.42-2.43 ms (TMA rows) vs 2.36-2.46 ms (lane loads), LMIP
+// 0.13-0.19 vs 0.10-0.11 ms — 128-byte bulk copies per thread are too small for the copy engine to
+// beat 32-bit lane loads here, and the rays are bound by the recurrence, not by the loads. The lane-load kernels stay the default; b2v_proj_set_tma(1) (or B2V_TMA=1) selects this path.
 int g_proj_tma = -1;
 inline bool tma_rows_ok(const void* vol, const Dims& d) {
   if (g_proj_tma < 0) g_proj_tma = getenv("B2V_TMA") != nullptr ? 1 : 0;

@@ -22,7 +22,7 @@ _KIND = {"max": _lib.MIP_MAX, "min": _lib.MIP_MIN, "mean": _lib.MIP_MEAN}
 
 def require_cuda() -> None:
     if not torch.cuda.is_available():
-        raise RuntimeError("invesalius3_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("invesalius3_b200 needs a CUDA device (sm_90a, H100); there is no CPU fallback")
 
 
 def _stream() -> C.c_void_p:
@@ -126,8 +126,8 @@ def d2h_async(src: torch.Tensor, out: np.ndarray) -> None:
 
 class _PinnedPool:
     """Recycled page-locked host blocks for result arrays. `tensor.cpu()` into fresh pageable
-    memory runs at ~2.6 GB/s (page faults + staged copies); a DMA into pinned memory runs at
-    PCIe rate (~55 GB/s), but cudaHostAlloc is slow, so blocks are pooled: a block returns
+    memory is slowed by page faults and staged copies; a DMA into pinned memory runs at PCIe
+    rate, but cudaHostAlloc is slow, so blocks are pooled: a block returns
     to the pool when the numpy array handed to the caller (and every view of it) is gone."""
 
     def __init__(self):

@@ -6,7 +6,7 @@ Same names, argument order, in-place output convention and error behaviour as
 already use (`import invesalius_rs as floodfill / mips`), see INTEGRATION.md.
 
 Every function packs its (possibly strided, memmap-backed) arguments into dense device
-tensors, runs the sm_100a kernels of libb2v.so and writes results back into the
+tensors, runs the sm_90a kernels of libb2v.so and writes results back into the
 caller's arrays. There is no CPU fallback.
 
 Error mapping (reference -> here):

@@ -1,5 +1,5 @@
 """do_watershed with the reference's signature (invesalius/data/watershed_process.py:19-60)
-on the sm_100a kernels of libb2v.so (b2v_ws_*), plus the device-level pieces.
+on the sm_90a kernels of libb2v.so (b2v_ws_*), plus the device-level pieces.
 
 Cost model and labelling rule: include/b2v.h (b2v_ws_flood) and DESIGN.md section 6. The
 LUT and the morphological gradient are bit-exact against NumPy / SciPy; the flood computes

@@ -4,8 +4,8 @@
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.c).
  *
- * scikit-image 0.24.0 is a third-party dependency that is absent from this image and from
- * /root/reference (pyproject.toml:35), so this follows its published algorithm
+ * scikit-image 0.24.0 is a third-party dependency of the reference (pyproject.toml:35) that
+ * is not vendored with it, so this follows its published algorithm
  * (skimage/segmentation/_watershed_cy.pyx::watershed_raveled + heap_general.pxi) from
  * memory — PARITY UNPINNED:
  *   - every marker voxel is pushed (raveled order) with key (value = image, age = 0);

@@ -25,17 +25,27 @@ def test_threshold_cranium_crop(orc, cranium):
         assert 0 < int((got == 255).sum()) < got.size
 
 
-def test_threshold_cranium_full_if_reference_present(orc, cranium):
-    """Whole-volume check against the shipped masks; only where /root/reference exists."""
-    import sys
+def test_threshold_cranium_full(orc, cranium):
+    """Whole-volume check against the shipped masks, on the Cranium matrix reduced to what
+    thresholding at their bounds can see (tools/make_golden_cranium.py:thr_matrix)."""
+    import io
+    import lzma
     from pathlib import Path
-    src = Path("/root/reference/samples/Cranium.inv3")
-    if not src.exists():
-        pytest.skip("reference checkout not present (GPU box)")
-    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tools"))
-    from make_golden_cranium import load_inv3
-    _, matrix, masks = load_inv3(src)
-    assert np.array_equal(matrix.astype(np.int64).sum(axis=(1, 2)), cranium["matrix_slice_sums"])
+    src = Path(__file__).resolve().parent / "golden" / "cranium_thr_matrix.npy.xz"
+    matrix = np.load(io.BytesIO(lzma.decompress(src.read_bytes())))
+    shape = tuple(cranium["full_shape"])
+    assert matrix.shape == shape and matrix.dtype == np.int16
+    # on the crop, the reduced matrix sits between the same threshold edges as the real one
+    crop = tuple(slice(a, b) for a, b in cranium["crop"])
+    edges = sorted({int(cranium[f"thr_{i}"][0]) for i in (0, 1)} | {int(cranium[f"thr_{i}"][1]) + 1 for i in (0, 1)})
+    assert np.array_equal(np.searchsorted(edges, matrix[crop], side="right"),
+                          np.searchsorted(edges, cranium["matrix_crop"], side="right"))
+    masks = []
+    for i in (0, 1):
+        bits = np.unpackbits(cranium[f"mask_{i}_bits_full"])[: matrix.size].reshape(shape)
+        m = np.zeros((shape[0] + 1, shape[1] + 1, shape[2] + 1), np.uint8)
+        m[1:, 1:, 1:] = bits * np.uint8(255)
+        masks.append((tuple(int(t) for t in cranium[f"thr_{i}"]), m))
     for i, (thr, m) in enumerate(masks):
         got = np.zeros(matrix.shape, np.uint8)
         orc.threshold(matrix, thr[0], thr[1], got, False)

@@ -1,4 +1,8 @@
-"""profiles/rNN_traffic.json from `ncu -i X.ncu-rep --page raw --csv` of ONE pipeline step (tools/step_once.py):
+"""Per-kernel and per-stage DRAM traffic of ONE pipeline step (tools/step_once.py), from the CSV of
+`ncu -i X.ncu-rep --page raw --csv`:
+
+    python tools/traffic_from_ncu.py <ncu.csv> <out.json> <V> <T>
+
 per kernel DRAM bytes + cold duration, per stage the sums next to the algorithmic bytes."""
 import csv, json, sys
 src, out, V, T = sys.argv[1], sys.argv[2], int(sys.argv[3]), int(sys.argv[4])
