@@ -255,6 +255,40 @@ int b2v_apply_view_matrix_transform(const void* volume, int dtype, int64_t dz, i
                                     int minterpol, double cval, void* out, int64_t odz, int64_t ody, int64_t odx,
                                     void* workspace, void* stream);
 
+/* ---- 3-D mask editor --------------------------------------------------------------------------
+ * The three crate functions behind invesalius/data/mask3d_editor_state.py:14. float64 in the
+ * reference's order; integer conversions as the crate's release build performs them.
+ * b2v_polygon2mask: invesalius_rs.polygon2mask_rs((w, h), polygon) (polygon_mask_py.rs:7-27 ->
+ *   polygon_mask.rs:4-79). polygon_host: n (x, y) float64 pairs on the HOST; out: dense [w][h] uint8,
+ *   1 inside and 0 outside (cell [r][c] is the screen point (r, c)); only the polygon's bounding box,
+ *   widened by one cell, is tested by the even-odd ray cast, every other cell is 0. A non-finite
+ *   vertex is B2V_ERR_ARG. workspace: >= 16 n bytes on the device.
+ * b2v_mask_cut: invesalius_rs.mask_cut(image, sx, sy, sz, max_depth, mask, M, MV, out, edit_mode)
+ *   (mask_cut_py.rs:8-69 -> mask_cut.rs:7-62). out: dense [dz][dy][dx] uint8, 16-byte aligned, edited in
+ *   place: a voxel > 127 at p = (x sx, y sy, z sz, 1) becomes 0 when M p has w > 0, |MV p / (MV p)_w|
+ *   <= max_depth, and either it projects onto the viewport where filter is non-zero or it projects
+ *   off the viewport and edit_mode == 0. filter: dense [h][w] uint8 (device). spacing_host = (sx, sy,
+ *   sz), m_host / mv_host = 16 doubles row-major, all on the HOST. The image is not needed.
+ * b2v_brush_mask_box: the brush's voxel box (brush_mask.rs:24-31) on the HOST: box_host = (z0, y0,
+ *   x0, z1, y1, x1), inclusive; (0, 0, 0, -1, -1, -1) when empty. b2v_brush_mask computes the same box.
+ * b2v_brush_mask: invesalius_rs.brush_mask_rs(out, orig, spacing, center, radius, edit_mode)
+ *   (brush_mask_py.rs:7-28 -> brush_mask.rs:5-71) on a [dz][dy][dx] volume with center_host = (cx, cy,
+ *   cz) in millimetres. out (and orig, or NULL) hold volume voxel (oz, oy, ox) at their first byte and
+ *   voxel (z, y, x) at (z - oz) plane_pitch + (y - oy) row_pitch + (x - ox); they must cover the box.
+ *   So the buffers may be the whole volume (origin 0) or a dense copy of just the box (origin z0, y0,
+ *   x0). Mode 1 zeroes voxels > 0 inside the sphere; mode 0 copies orig > 0 into it (255 without
+ *   orig); any other mode does nothing. */
+int b2v_polygon2mask(const double* polygon_host, int64_t n, int64_t w, int64_t h, uint8_t* out, void* workspace,
+                     void* stream);
+int b2v_mask_cut(uint8_t* out, int64_t dz, int64_t dy, int64_t dx, const double* spacing_host, double max_depth,
+                 const uint8_t* filter, int64_t h, int64_t w, const double* m_host, const double* mv_host, int edit_mode,
+                 void* stream);
+int b2v_brush_mask_box(int64_t dz, int64_t dy, int64_t dx, const double* spacing_host, const double* center_host,
+                       double radius, int64_t* box_host);
+int b2v_brush_mask(uint8_t* out, const uint8_t* orig, int64_t dz, int64_t dy, int64_t dx, int64_t oz, int64_t oy,
+                   int64_t ox, int64_t row_pitch, int64_t plane_pitch, const double* spacing_host,
+                   const double* center_host, double radius, int edit_mode, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

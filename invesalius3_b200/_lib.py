@@ -98,6 +98,10 @@ PROTOTYPES = {
     "b2v_peer_mc_inbox_offset": (i64, [i64, u32]),
     "b2v_mida_z_partial": (cint, [vp, cint, i64, i64, i64, dbl, dbl, vp, vp, cint, cint, vp, cint, vp, vp]),
     "b2v_lmip_z_partial": (cint, [vp, cint, i64, i64, i64, dbl, dbl, vp, cint, cint, vp, vp, vp]),
+    "b2v_polygon2mask": (cint, [vp, i64, i64, i64, vp, vp, vp]),
+    "b2v_mask_cut": (cint, [vp, i64, i64, i64, vp, dbl, vp, i64, i64, vp, vp, cint, vp]),
+    "b2v_brush_mask_box": (cint, [i64, i64, i64, vp, vp, dbl, C.POINTER(i64)]),
+    "b2v_brush_mask": (cint, [vp, vp, i64, i64, i64, i64, i64, i64, i64, i64, vp, vp, dbl, cint, vp]),
 }
 
 _lib = None
