@@ -289,6 +289,29 @@ int b2v_brush_mask(uint8_t* out, const uint8_t* orig, int64_t dz, int64_t dy, in
                    int64_t ox, int64_t row_pitch, int64_t plane_pitch, const double* spacing_host,
                    const double* center_host, double radius, int edit_mode, void* stream);
 
+/* ---- region growing -----------------------------------------------------------------------------
+ * The "Region growing" tool (invesalius/data/styles.py:2991-3251) and Slice.calc_image_density
+ * (slice_.py:2284-2297).
+ * b2v_lut255: get_LUT_value_255(data, window, level) (imagedata_utils.py:540-552) over n voxels of
+ *   dtype B2V_I16 / B2V_U8 / B2V_F64; out has the input's dtype (integers truncate, as a C cast does).
+ *   float64 arithmetic in NumPy's order; where the two conditions overlap (window <= 1) 255 wins.
+ * b2v_masked_moments: count, min, max, np.mean and np.std (bit-identical: NumPy's pairwise summation
+ *   order) of the image's voxels in the selection: sel[i] == sel_value (B2V_SEL_EQ) or sel[i] > 127
+ *   (B2V_SEL_GT127) on a dense uint8 [dz][dy][dx] sel (or NULL: none), OR the voxel box box_host =
+ *   (z0, y0, x0, z1, y1, x1) on the HOST, inclusive, clipped to the volume (or NULL: none). stats_host
+ *   is written on the host; count 0 leaves min, max, mean and std NaN. Synchronises the stream.
+ *   workspace: b2v_masked_moments_workspace_bytes(dz, dy, dx) bytes on the device. */
+#define B2V_SEL_EQ 0
+#define B2V_SEL_GT127 1
+typedef struct b2v_moments {
+  int64_t count;
+  double min, max, mean, std;
+} b2v_moments;
+int b2v_lut255(const void* img, int dtype, int64_t n, double window, double level, void* out, void* stream);
+int64_t b2v_masked_moments_workspace_bytes(int64_t dz, int64_t dy, int64_t dx);
+int b2v_masked_moments(const void* img, int dtype, int64_t dz, int64_t dy, int64_t dx, const uint8_t* sel, int sel_mode,
+                       int sel_value, const int64_t* box_host, b2v_moments* stats_host, void* workspace, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

@@ -102,7 +102,17 @@ PROTOTYPES = {
     "b2v_mask_cut": (cint, [vp, i64, i64, i64, vp, dbl, vp, i64, i64, vp, vp, cint, vp]),
     "b2v_brush_mask_box": (cint, [i64, i64, i64, vp, vp, dbl, C.POINTER(i64)]),
     "b2v_brush_mask": (cint, [vp, vp, i64, i64, i64, i64, i64, i64, i64, i64, vp, vp, dbl, cint, vp]),
+    "b2v_lut255": (cint, [vp, cint, i64, dbl, dbl, vp, vp]),
+    "b2v_masked_moments_workspace_bytes": (i64, [i64, i64, i64]),
+    "b2v_masked_moments": (cint, [vp, cint, i64, i64, i64, vp, cint, cint, vp, vp, vp, vp]),
 }
+
+SEL_EQ, SEL_GT127 = 0, 1
+
+
+class Moments(C.Structure):
+    """b2v_moments of include/b2v.h."""
+    _fields_ = [("count", i64), ("min", dbl), ("max", dbl), ("mean", dbl), ("std", dbl)]
 
 _lib = None
 
