@@ -1160,10 +1160,11 @@ int persistent_verdict(const Workspace& w, cudaStream_t s) {
   return B2V_OK;
 }
 
-// verdict_later: the caller queues more work behind the kernel and calls persistent_verdict()
-// itself (one host round trip per flood instead of two).
+// *verdict_later: the caller queues more work behind the kernel and calls persistent_verdict()
+// itself (one host round trip per flood instead of two). Cleared when the host-driven rounds ran
+// instead: they have checked convergence already, and the unlaunched kernel's verdict would report 0 rounds.
 int run_persistent(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_t s, int r0, int* rounds_out,
-                   bool verdict_later, const PeerSet* peer = nullptr) {
+                   bool* verdict_later, const PeerSet* peer = nullptr) {
   int ntiles = b.ntz * b.nty * b.ntw;
   const size_t smem = 2 * (size_t)(b.tz + 2) * (b.ty + 2) * (b.tw + 2) * sizeof(uint32_t);
   int rc;
@@ -1190,6 +1191,7 @@ int run_persistent(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_
   // a block keeps at most kMaxMine tiles of a round in shared memory (4.4 G voxels at 132 blocks and 16^3-word tiles)
   if ((int64_t)grid * kMaxMine < ntiles) {
     B2V_REQUIRE(!peer, B2V_ERR_ARG, "floodfill: shard too large for the fused peer exchange (%d tiles)", ntiles);
+    *verdict_later = false;
     return run_rounds(b, w, sb, s, r0, rounds_out);
   }
   k_ff_lists_init<<<1, 1024, 0, s>>>(w.active[r0 & 1], w.active[r0 & 1], (int)ntiles, bm, nbw);
@@ -1208,7 +1210,7 @@ int run_persistent(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_
   // the round flag of r0 was consumed; the next merge raises flags[r0 + 1]
   B2V_CUDA(cudaMemsetAsync(w.flags + r0, 0, sizeof(int), s));
   if (rounds_out) *rounds_out = r0 + 1;
-  return verdict_later ? B2V_OK : persistent_verdict(w, s);
+  return *verdict_later ? B2V_OK : persistent_verdict(w, s);
 }
 
 enum { STAGE_BEGIN = 1, STAGE_CONVERGE = 2, STAGE_FINISH = 4, STAGE_ALL = 7 };
@@ -1263,7 +1265,7 @@ int flood(T* data, uint8_t* out, int64_t dz, int64_t dy, int64_t dx, const int64
       B2V_REQUIRE(b.dz >= 2 && b.dy * (int64_t)b.wx * 4 <= peer->pc, B2V_ERR_ARG,
                   "floodfill: the shard's planes do not fit the peer mailboxes (or the slab has < 2 planes)");
     }
-    if ((rc = (g_flood_engine || peer) ? run_persistent(b, w, sb, s, r0, &r1, verdict_due, peer)
+    if ((rc = (g_flood_engine || peer) ? run_persistent(b, w, sb, s, r0, &r1, &verdict_due, peer)
                                        : run_rounds(b, w, sb, s, r0, &r1)))
       return rc;
     if (round_io) *round_io = r1;

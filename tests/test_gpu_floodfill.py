@@ -302,8 +302,8 @@ def test_floodfill_wide_rows_many_x_tiles(rs, orc):
 def test_floodfill_canonical_tiles_across_x(rs, orc, shape):
     """The 6-connected fast path on 16 x 16 x 16-word tiles with several tiles along x (rows
     wider than 512 voxels), partial tiles on every side: the run fill has to cross word and
-    tile boundaries through the halo words. Also in place and with the small-tile knob."""
-    import os
+    tile boundaries through the halo words. Also in place. (The small tiles of B2V_FF_TILE=8
+    need a process of their own: test_gpu_floodfill_paths.py.)"""
     rng = np.random.default_rng(31)
     # long thin structures along x so that the flood travels through many x tiles
     data = (ndimage.gaussian_filter(rng.normal(size=shape), (1.5, 1.5, 12)) > 0.0).astype(np.int16) * 1000
@@ -313,14 +313,9 @@ def test_floodfill_canonical_tiles_across_x(rs, orc, shape):
     want = np.zeros(shape, np.uint8)
     orc.floodfill_threshold(data, seeds, 500, 1500, 200, st, want)
     assert (want == 200).sum() > 5000
-    for knob in (None, "8"):
-        if knob: os.environ["B2V_FF_TILE"] = knob
-        try:
-            got = np.zeros(shape, np.uint8)
-            rs.floodfill_threshold(data, seeds, 500, 1500, 200, st, got)
-        finally:
-            os.environ.pop("B2V_FF_TILE", None)
-        assert np.array_equal(got, want), knob
+    got = np.zeros(shape, np.uint8)
+    rs.floodfill_threshold(data, seeds, 500, 1500, 200, st, got)
+    assert np.array_equal(got, want)
     mask = (data > 0).astype(np.uint8) * 255
     want_ip = mask.copy(); got_ip = mask.copy()
     orc.floodfill_threshold_inplace(want_ip, seeds, 255, 255, 7, st)
