@@ -312,6 +312,28 @@ int64_t b2v_masked_moments_workspace_bytes(int64_t dz, int64_t dy, int64_t dx);
 int b2v_masked_moments(const void* img, int dtype, int64_t dz, int64_t dy, int64_t dx, const uint8_t* sel, int sel_mode,
                        int sel_value, const int64_t* box_host, b2v_moments* stats_host, void* workspace, void* stream);
 
+/* ---- spline resampling ------------------------------------------------------------------------------
+ * b2v_zoom: scipy.ndimage.zoom(input, zoom, output, order, mode, cval) with prefilter=True and
+ * grid_mode=False, as imagedata_utils.resize_image_array / resize_slice call it (order 2,
+ * imagedata_utils.py:109-129; surface.py:1352-1353) and as the DICOM preview and the thumbnails do (order
+ * 3, :132-139, :271-284). in: dense [nz][ny][nx] of in_dtype (B2V_I16, B2V_U8, B2V_F32, B2V_F64); ndim 2
+ * for a 2-D image (passed with nz = out_nz = 1), 3 for a volume (SciPy's 3-D sum differs from the 2-D one
+ * even where nz is 1). out: dense [out_nz][out_ny][out_nx] of out_dtype. order 0-3; orders 2 and 3 first
+ * run SciPy's spline prefilter into the float64 workspace (b2v_zoom_workspace_bytes: 8 B per input voxel,
+ * 0 for orders 0 and 1). Output index o samples o * (n_in - 1) / (n_out - 1) (1 when n_out is 1); taps past
+ * an edge fold by mirror. mode B2V_ZOOM_CONSTANT: a coordinate that rounds past n_in - 1 writes cval
+ * (SciPy's test is strict); B2V_ZOOM_MIRROR: it is interpolated. Integer outputs round half away from zero
+ * and clip to their range; float outputs take the float64 value's cast. float64, SciPy's evaluation order:
+ * bit-exact. Algorithmic bytes, orders 2 and 3: 3 reads + 2 writes of 8 B per voxel and axis (the z pass
+ * reads the input dtype), then the gather (its taps mostly hit cache: ~8 B per input voxel read, out
+ * written once). */
+#define B2V_F32 3
+#define B2V_ZOOM_CONSTANT 0
+#define B2V_ZOOM_MIRROR 1
+int64_t b2v_zoom_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order);
+int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int64_t ny, int64_t nx, int64_t out_nz, int64_t out_ny,
+             int64_t out_nx, int order, int mode, double cval, void* out, int out_dtype, void* workspace, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

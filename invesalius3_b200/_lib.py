@@ -105,7 +105,12 @@ PROTOTYPES = {
     "b2v_lut255": (cint, [vp, cint, i64, dbl, dbl, vp, vp]),
     "b2v_masked_moments_workspace_bytes": (i64, [i64, i64, i64]),
     "b2v_masked_moments": (cint, [vp, cint, i64, i64, i64, vp, cint, cint, vp, vp, vp, vp]),
+    "b2v_zoom_workspace_bytes": (i64, [i64, i64, i64, cint]),
+    "b2v_zoom": (cint, [vp, cint, cint, i64, i64, i64, i64, i64, i64, cint, cint, dbl, vp, cint, vp, vp]),
 }
+
+F32 = 3
+ZOOM_CONSTANT, ZOOM_MIRROR = 0, 1
 
 SEL_EQ, SEL_GT127 = 0, 1
 
