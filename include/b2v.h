@@ -215,7 +215,8 @@ int b2v_uniform_filter_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx
  * for jj = -radius .. -1: tmp += (x[c + jj] +/- x[c - jj]) w[jj]; float64; 'reflect'; an int16 output
  * takes the C cast. weights_dev: 2 radius + 1 centred float64 weights on the device (for a Gaussian:
  * scipy.ndimage._filters._gaussian_kernel1d, reversed). dtype pairs (int16,int16), (int16,float64),
- * (float64,float64). b2v_sharpen_i16, b2v_sobel_magnitude, b2v_rescale_cast_i16: the elementwise
+ * (float64,float64), (float32,float32) (the sum stays float64 and is rounded to float, as SciPy's line
+ * buffer does). b2v_sharpen_i16, b2v_sobel_magnitude, b2v_rescale_cast_i16: the elementwise
  * float64 statements around them, in NumPy's order. Bit-exact against SciPy. */
 int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t ny, int64_t nx, int axis, const double* weights_dev,
                     int radius, int symmetry, void* out, int out_dtype, void* stream);
@@ -333,6 +334,39 @@ int b2v_masked_moments(const void* img, int dtype, int64_t dz, int64_t dy, int64
 int64_t b2v_zoom_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order);
 int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int64_t ny, int64_t nx, int64_t out_nz, int64_t out_ny,
              int64_t out_nx, int order, int mode, double cval, void* out, int out_dtype, void* workspace, void* stream);
+
+/* ---- porous scaffolds: Voronoi ---------------------------------------------------------------------
+ * The "Voronoi" scaffolds of the porous-creation plugin (plugins/porous_creation/schwarzp.py:37-84).
+ * b2v_jump_flooding: invesalius_rs.jump_flooding(distance_map, map_owners, sites, normalize)
+ *   (floodfill_py.rs:262-276 -> floodfill.rs:298-507), in place on dense [dz][dy][dx] float32 distances and
+ *   int32 owners. sites: dense int32 [n_sites][3] (z, y, x) on the device. Site i seeds owner i + 1 and
+ *   distance 0 at its voxel (the last site naming a voxel wins; a negative or out-of-range site seeds
+ *   nothing). Then floor(log2(max(dz, dy, dx))) Jacobi steps with per-axis offsets size / 2, halved after
+ *   every step: each voxel takes the neighbour owner (1 .. n_sites) whose site is strictly nearer, in float32
+ *   sqrt((dz dz + dy dy) + dx dx), or the first one when it has no owner (owner <= 0). normalize != 0 then
+ *   replaces every distance of a voxel owned by 1 .. n_sites by its distance to the owner's truncated
+ *   centroid over that site's largest such distance (when > 0). n_sites == 0 or an empty volume returns
+ *   untouched. Shapes of more than 2^32 - 1 voxels with normalize (the crate's u32 per-site counts could
+ *   wrap), more than 2^31 - 2 sites or dims beyond the grid are B2V_ERR_ARG. workspace:
+ *   b2v_jump_flooding_workspace_bytes (a second owner and distance volume, 8 B per voxel, and 64 B per site).
+ *   Algorithmic bytes per step: 16 B per voxel compulsory (owner and distance read and written) and 104 B
+ *   gathered (26 neighbour owners); normalize adds 12 B per voxel.
+ * b2v_voronoi_borders: mag > 0 of the owners' np.gradient (schwarzp.py:43-49): out[v] = 1.0f where the
+ *   integer owner difference along any differentiated axis is non-zero (central in the interior, one-sided
+ *   at the ends), else 0.0f. planar != 0: y and x only, dz must be 1 (the 2-D preview); planar == 0: all
+ *   three axes. Every differentiated axis needs >= 2 voxels (NumPy raises otherwise): B2V_ERR_ARG.
+ *   4 B read + 4 B written per voxel (the neighbours hit cache).
+ * b2v_image_normalize_f32_i16: imagedata_utils.image_normalize(image, min_, max_) for a float32 image and an
+ *   int16 output (imagedata_utils.py:580-587, plugins/porous_creation/gui.py:237): out = C cast of
+ *   (in - imin) * (span / (imax - imin)) + min_f, all float32 (span = float32(max_ - min_), min_f =
+ *   float32(min_), as NumPy promotes Python scalars against float32); `fill` everywhere when imin == imax.
+ *   imin / imax: the image's minimum and maximum. 4 B read + 2 B written per voxel. */
+int64_t b2v_jump_flooding_workspace_bytes(int64_t dz, int64_t dy, int64_t dx, int64_t n_sites);
+int b2v_jump_flooding(float* distance_map, int32_t* map_owners, int64_t dz, int64_t dy, int64_t dx, const int32_t* sites,
+                      int64_t n_sites, int normalize, void* workspace, void* stream);
+int b2v_voronoi_borders(const int32_t* owners, int64_t dz, int64_t dy, int64_t dx, int planar, float* out, void* stream);
+int b2v_image_normalize_f32_i16(const float* in, int64_t n, float imin, float imax, float span, float min_f,
+                                int16_t fill, int16_t* out, void* stream);
 
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:

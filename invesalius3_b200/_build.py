@@ -79,9 +79,9 @@ def build_cuda(force: bool = False, verbose: bool = False) -> Path:
 
 
 def build_oracle(force: bool = False) -> Path:
-    """Compile the CPU oracle (test infrastructure only) via oracle/Makefile, and the 3-D mask
-    editor's checker via oracle/editor.mk."""
-    for makefile in ([], ["-f", "editor.mk"]):
+    """Compile the CPU oracle (test infrastructure only) via oracle/Makefile, the 3-D mask
+    editor's checker via oracle/editor.mk and the jump-flooding checker via oracle/voronoi.mk."""
+    for makefile in ([], ["-f", "editor.mk"], ["-f", "voronoi.mk"]):
         r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *makefile, *(["-B"] if force else [])],
                            capture_output=True, text=True)
         if r.returncode != 0:

@@ -107,6 +107,10 @@ PROTOTYPES = {
     "b2v_masked_moments": (cint, [vp, cint, i64, i64, i64, vp, cint, cint, vp, vp, vp, vp]),
     "b2v_zoom_workspace_bytes": (i64, [i64, i64, i64, cint]),
     "b2v_zoom": (cint, [vp, cint, cint, i64, i64, i64, i64, i64, i64, cint, cint, dbl, vp, cint, vp, vp]),
+    "b2v_jump_flooding_workspace_bytes": (i64, [i64, i64, i64, i64]),
+    "b2v_jump_flooding": (cint, [vp, vp, i64, i64, i64, vp, i64, cint, vp, vp]),
+    "b2v_voronoi_borders": (cint, [vp, i64, i64, i64, cint, vp, vp]),
+    "b2v_image_normalize_f32_i16": (cint, [vp, i64, f32, f32, f32, f32, C.c_int16, vp, vp]),
 }
 
 F32 = 3

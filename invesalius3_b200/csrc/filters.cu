@@ -32,6 +32,7 @@ __device__ __forceinline__ long long reflect_idx(long long i, long long n) {   /
 template <typename TO> __device__ __forceinline__ TO cast_out(double v);
 template <> __device__ __forceinline__ int16_t cast_out<int16_t>(double v) { return (int16_t)(int)v; }
 template <> __device__ __forceinline__ double cast_out<double>(double v) { return v; }
+template <> __device__ __forceinline__ float cast_out<float>(double v) { return (float)v; }
 
 // op: 0 union, 1 difference, 2 intersection, 3 xor; selected <=> value > 2 (slice_.py:1906-1916)
 __global__ void __launch_bounds__(256) k_boolean_op(const uint8_t* __restrict__ m1, const uint8_t* __restrict__ m2, long long n,
@@ -241,7 +242,7 @@ extern "C" int b2v_uniform_filter_i16(const int16_t* in, int64_t nz, int64_t ny,
   return b2v_check_launch("k_uniform1d_i16");
 }
 
-// dtype codes: B2V_I16 or B2V_F64 for input and output; in != out
+// dtype pairs (B2V_I16, B2V_I16), (B2V_I16, B2V_F64), (B2V_F64, B2V_F64), (B2V_F32, B2V_F32); in != out
 extern "C" int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t ny, int64_t nx, int axis,
                                const double* weights_dev, int radius, int symmetry, void* out, int out_dtype, void* stream) {
   B2V_REQUIRE(in && out && in != out && weights_dev && nz > 0 && ny > 0 && nx > 0 && axis >= 0 && axis <= 2 && radius >= 0 &&
@@ -256,7 +257,9 @@ extern "C" int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t
     k_correlate1d<int16_t, double><<<g, 256, 0, s>>>((const int16_t*)in, (int)nz, (int)ny, (int)nx, axis, weights_dev, radius, symmetry, (double*)out);
   else if (in_dtype == B2V_F64 && out_dtype == B2V_F64)
     k_correlate1d<double, double><<<g, 256, 0, s>>>((const double*)in, (int)nz, (int)ny, (int)nx, axis, weights_dev, radius, symmetry, (double*)out);
-  else B2V_REQUIRE(false, B2V_ERR_ARG, "correlate1d: dtype pair must be (int16,int16), (int16,float64) or (float64,float64)");
+  else if (in_dtype == B2V_F32 && out_dtype == B2V_F32)
+    k_correlate1d<float, float><<<g, 256, 0, s>>>((const float*)in, (int)nz, (int)ny, (int)nx, axis, weights_dev, radius, symmetry, (float*)out);
+  else B2V_REQUIRE(false, B2V_ERR_ARG, "correlate1d: dtype pair must be (int16,int16), (int16,float64), (float64,float64) or (float32,float32)");
   return b2v_check_launch("k_correlate1d");
 }
 

@@ -59,7 +59,7 @@ def _corr(t: torch.Tensor, axis: int, weights: np.ndarray, symmetry: int, out_dt
     """One scipy.ndimage.correlate1d pass (b2v_correlate1d) on a device volume."""
     w = torch.from_numpy(np.ascontiguousarray(weights, dtype=np.float64)).to(t.device)
     out = torch.empty(t.shape, dtype=out_dtype, device=t.device)
-    code = {torch.int16: _lib.I16, torch.float64: _lib.F64}
+    code = {torch.int16: _lib.I16, torch.float64: _lib.F64, torch.float32: _lib.F32}
     with torch.cuda.device(t.device):
         _lib.call("b2v_correlate1d", _p(t), code[t.dtype], *t.shape, axis, _p(w), len(weights) // 2, symmetry, _p(out),
                   code[out_dtype], _stream())
