@@ -149,10 +149,6 @@ int b2v_fill_holes(uint8_t* mask, const uint32_t* labels, int64_t n, uint32_t nl
  * is B2V_ERR_ARG ("Invalid image or output type"). wl / ww are taken AS THE IMAGE TYPE
  * (mips_py.rs:174-175). 4 B/voxel for int16 (min/max pass + ray pass). */
 int64_t b2v_proj_workspace_bytes(int64_t n);
-/* rays along x of int16 volumes: 1 = rows staged by the TMA engine (cp.async.bulk + mbarrier, two
- * stages), 0 = 32-bit lane loads through a padded shared-memory tile (default: as fast for MIDA and
- * faster for LMIP on the H100, see proj.cu). Process-wide, like b2v_floodfill_set_engine. */
-void b2v_proj_set_tma(int on);
 int b2v_mida(const void* img, int dtype, int64_t dz, int64_t dy, int64_t dx, int axis, double wl, double ww,
              void* out, int out_dtype, void* workspace, void* stream);
 /* same, with the (min, max) pair of mips.rs:113-122 supplied by the caller as float[2] on

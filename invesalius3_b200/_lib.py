@@ -43,7 +43,6 @@ PROTOTYPES = {
     "b2v_fill_holes_staged": (cint, [cint, vp, vp, i64, u32, u32, vp, vp, C.POINTER(cint)]),
     "b2v_fill_holes": (cint, [vp, vp, i64, u32, u32, vp, vp, C.POINTER(cint)]),
     "b2v_proj_workspace_bytes": (i64, [i64]),
-    "b2v_proj_set_tma": (None, [cint]),
     "b2v_mida": (cint, [vp, cint, i64, i64, i64, cint, dbl, dbl, vp, cint, vp, vp]),
     "b2v_mida_minmax": (cint, [vp, cint, i64, i64, i64, cint, dbl, dbl, vp, vp, cint, vp, vp]),
     "b2v_lmip": (cint, [vp, cint, i64, i64, i64, cint, dbl, dbl, vp, vp, vp]),

@@ -8,17 +8,18 @@
 // (explicit __f*_rn intrinsics); casts to the output type truncate toward zero and a value
 // that does not fit (NaN included) is reported as B2V_ERR_RANGE, where the reference panics.
 //
-// One ray per thread. Rays along z or y (axis 0/1) keep x contiguous across the threads
-// of a warp, so every step is a coalesced row access; rays along x (axis 2) are staged
-// through a padded shared-memory tile (128 rays x 32 samples) that is loaded row-wise
-// (coalesced) and walked column-wise (bank-conflict free). A block stops loading as soon
-// as all of its rays have terminated (alpha >= 1 in MIDA, first local maximum in LMIP).
+// One ray per thread; MIDA and LMIP are operators (MidaOp, LmipOp) run by the same ray kernels.
+// Rays along z or y (axis 0/1) keep x contiguous across the threads of a warp, so every step is
+// a coalesced row access; rays along x (axis 2) are staged through a padded shared-memory tile
+// (128 rays x 32 samples) that is loaded row-wise (coalesced) and walked column-wise (bank-conflict
+// free). A block stops loading as soon as all of its rays have terminated (alpha >= 1 in MIDA,
+// first local maximum in LMIP).
 // HBM: 2 B/voxel for the ray pass + 2 B/voxel for the global min/max pass MIDA needs.
 //
-// The contour variants never materialise the reference's temp volume: a sampler computes
-// the T-typed contour intensity of a voxel on the fly from its six neighbours.
+// The contour variants do as the reference does: k_fcm_volume materialises the contour volume,
+// which b2v_mip, b2v_lmip or b2v_mida then projects. The *_z_partial entry points walk the rays
+// along z through one Z shard at a time, handing each ray's state on to the next shard.
 #include <math.h>
-#include <stdlib.h>
 
 #include "b2v_common.cuh"
 
@@ -26,18 +27,6 @@ namespace {
 
 struct Dims {
   int64_t nz, ny, nx;
-};
-
-// ---- samplers -----------------------------------------------------------------------------
-template <typename T>
-struct PlainSampler {
-  static constexpr int kBatch = 8;   // samples fetched ahead of the recurrence (plain loads)
-  static constexpr bool kLinear = true;   // a sample is vol[flat index]: rays advance a pointer
-  const T* __restrict__ vol;
-  Dims d;
-  __device__ __forceinline__ T at(int64_t z, int64_t y, int64_t x, int* status) const {
-    return vol[(z * d.ny + y) * d.nx + x];
-  }
 };
 
 template <typename T> __device__ __forceinline__ float wrapdiff(T a, T b);
@@ -69,6 +58,10 @@ template <> __device__ __forceinline__ bool cast_f32<uint8_t>(float f, uint8_t* 
 }
 
 // ---- per-ray operators --------------------------------------------------------------------
+// An operator is copied into every thread, which calls init() once, first() with the ray's first
+// sample, step() with every sample from the first on until it reports the ray finished, and
+// result() at the end.
+
 // get_opacity (mips.rs:88-100). The window bounds are ray-invariant: computed once per thread
 // (same float32 operations, so the same values) instead of once per sample.
 struct Window {
@@ -88,10 +81,18 @@ struct Window {
 
 template <typename T, typename U>
 struct MidaOp {
-  float img_min, range, inv, wl, ww;
+  // The (min, max) pair of the volume stays on the device (b2v_minmax_f32 or the caller wrote
+  // it): every thread derives (min, range, 1/range) from it in init() instead of the host
+  // synchronising to read it.
+  const float* mm;
+  float wl, ww;
+  float img_min, range, inv;
   float fmax, alpha_p, colour_p, final_colour;
   Window win;
   __device__ __forceinline__ void init() {
+    img_min = mm[0];
+    range = __fsub_rn(mm[1], mm[0]);
+    inv = __fdiv_rn(1.0f, range);
     fmax = alpha_p = colour_p = final_colour = 0.0f;
     win.set(wl, ww);
   }
@@ -181,95 +182,69 @@ struct LmipOp {
   }
 };
 
-template <typename T>
-struct MaxOp {  // fold_axis with Bounded::min_value() (mips.rs:250-254)
-  T m;
-  __device__ __forceinline__ void init() {}
-  __device__ __forceinline__ void first(T v) { m = v; }
-  __device__ __forceinline__ bool step(T v) {
-    if (v > m) m = v;
-    return false;
-  }
-  __device__ __forceinline__ bool result(T* o) const {
-    *o = m;
-    return true;
-  }
-};
+// ---- ray kernels ---------------------------------------------------------------------------
+// One ray of a keep-x kernel (axis 0: along z, axis 1: along y): a pointer advanced by a constant
+// stride. kBatch samples are fetched before any of them is consumed, because the recurrence is a
+// long dependent chain the loads must not wait for. The walk stops at the first sample whose
+// step() reports the ray finished.
+constexpr int kBatch = 8;
 
-// ---- ray walkers ---------------------------------------------------------------------------
-// One ray of a keep-x kernel (axis 0: along z, axis 1: along y). For a plain volume the ray is
-// a pointer advanced by a constant stride; kBatch samples are fetched before any of them is
-// consumed, because the recurrence is a long dependent chain the loads must not wait for. The
-// walk stops at the first sample whose step() reports the ray finished.
-template <typename T, typename S, typename Op>
-__device__ __forceinline__ bool walk_keepx(const S& smp, int axis, int64_t r, int64_t x, int64_t n_l, Op& op, int* st) {
-  if constexpr (S::kLinear) {
-    constexpr int B = S::kBatch;
-    const int64_t plane = smp.d.ny * smp.d.nx;
-    const int64_t stride = axis == 0 ? plane : smp.d.nx;
-    const T* __restrict__ p = smp.vol + (axis == 0 ? r * smp.d.nx + x : r * plane + x);
-    int64_t l0 = 0;
-    for (; l0 + B <= n_l; l0 += B) {
-      T v[B];
+template <typename T, typename Op>
+__device__ __forceinline__ bool walk_keepx(const T* __restrict__ vol, Dims d, int axis, int64_t r, int64_t x,
+                                           int64_t n_l, Op& op) {
+  const int64_t plane = d.ny * d.nx;
+  const int64_t stride = axis == 0 ? plane : d.nx;
+  const T* __restrict__ p = vol + (axis == 0 ? r * d.nx + x : r * plane + x);
+  int64_t l0 = 0;
+  for (; l0 + kBatch <= n_l; l0 += kBatch) {
+    T v[kBatch];
 #pragma unroll
-      for (int k = 0; k < B; ++k) v[k] = p[k * stride];
-      p += B * stride;
+    for (int k = 0; k < kBatch; ++k) v[k] = p[k * stride];
+    p += kBatch * stride;
 #pragma unroll
-      for (int k = 0; k < B; ++k)
-        if (op.step(v[k])) return true;
-    }
-    for (; l0 < n_l; ++l0, p += stride)
-      if (op.step(*p)) return true;
-  } else {
-    for (int64_t l = 0; l < n_l; ++l) {
-      const T v = axis == 0 ? smp.at(l, r, x, st) : smp.at(r, l, x, st);
-      if (op.step(v)) return true;
-    }
+    for (int k = 0; k < kBatch; ++k)
+      if (op.step(v[k])) return true;
   }
+  for (; l0 < n_l; ++l0, p += stride)
+    if (op.step(*p)) return true;
   return false;
 }
 
 // axis 0: out[y][x], ray along z; axis 1: out[z][x], ray along y. One thread per (r, x).
-template <typename T, typename U, typename S, typename Op>
-__global__ void __launch_bounds__(128) k_rays_keepx(S smp, int axis, Op op0, U* __restrict__ out, int* status) {
-  const Dims d = smp.d;
+template <typename T, typename U, typename Op>
+__global__ void __launch_bounds__(128) k_rays_keepx(const T* __restrict__ vol, Dims d, int axis, Op op0,
+                                                    U* __restrict__ out, int* status) {
   const int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t r = blockIdx.y;
   if (x >= d.nx) return;
   const int64_t n_l = axis == 0 ? d.nz : d.ny;
   Op op = op0;
   op.init();
-  int st = 0;
-  {
-    T v0 = axis == 0 ? smp.at(0, r, x, &st) : smp.at(r, 0, x, &st);
-    op.first(v0);
-  }
-  walk_keepx<T>(smp, axis, r, x, n_l, op, &st);
+  op.first(vol[axis == 0 ? r * d.nx + x : r * d.ny * d.nx + x]);
+  walk_keepx<T>(vol, d, axis, r, x, n_l, op);
   U o;
-  if (op.result(&o)) out[r * d.nx + x] = o; else st = B2V_ERR_RANGE;
-  if (st) *status = st;
+  if (op.result(&o)) out[r * d.nx + x] = o; else *status = B2V_ERR_RANGE;
 }
 
 // axis 2: out[z][y], ray along x. 128 rays per block, 32 samples per tile.
 constexpr int kRays = 128, kChunk = 32;
-template <typename T> struct Pitch { static constexpr int value = kChunk + 4 / sizeof(T) * 1; };
+template <typename T> struct Pitch;
 template <> struct Pitch<int16_t> { static constexpr int value = kChunk + 2; };   // 17 words
 template <> struct Pitch<uint8_t> { static constexpr int value = kChunk + 4; };   // 9 words
 template <> struct Pitch<double> { static constexpr int value = kChunk + 1; };
 
-// Stage the 32-sample segments [x0, x0+32) of kRays consecutive rows in shared memory. A plain
-// int16 volume with even rows moves two samples per lane (half a warp per row, 64 B each);
-// otherwise one sample per lane (a warp per row), through the sampler.
-template <typename T, typename S>
-__device__ __forceinline__ void load_tile(const S& smp, T (*tile)[Pitch<T>::value], int64_t row0, int64_t nrows,
-                                          int64_t x0, int lane, int warp, int* st) {
-  const Dims d = smp.d;
-  if constexpr (S::kLinear && sizeof(T) == 2) {
-    if ((d.nx & 1) == 0 && (reinterpret_cast<uintptr_t>(smp.vol) & 3) == 0) {
+// Stage the 32-sample segments [x0, x0+32) of kRays consecutive rows in shared memory. An int16
+// volume with even rows moves two samples per lane (half a warp per row, 64 B each); otherwise
+// one sample per lane (a warp per row).
+template <typename T>
+__device__ __forceinline__ void load_tile(const T* __restrict__ vol, Dims d, T (*tile)[Pitch<T>::value], int64_t row0,
+                                          int64_t nrows, int64_t x0, int lane, int warp) {
+  if constexpr (sizeof(T) == 2) {
+    if ((d.nx & 1) == 0 && (reinterpret_cast<uintptr_t>(vol) & 3) == 0) {
       const int half = lane >> 4, l16 = lane & 15;
       const int64_t x = x0 + 2 * l16;
       const bool xin = x < d.nx;
-      const T* p = smp.vol + (row0 + warp * 2 + half) * d.nx + x;
+      const T* p = vol + (row0 + warp * 2 + half) * d.nx + x;
       const int64_t step = (int64_t)(kRays / 16) * d.nx;
 #pragma unroll
       for (int rr = warp * 2 + half; rr < kRays; rr += kRays / 16, p += step) {
@@ -284,14 +259,7 @@ __device__ __forceinline__ void load_tile(const S& smp, T (*tile)[Pitch<T>::valu
     const int64_t row = row0 + rr;
     const int64_t x = x0 + lane;
     T v = 0;
-    if (row < nrows && x < d.nx) {
-      if constexpr (S::kLinear) {
-        v = smp.vol[row * d.nx + x];
-      } else {
-        const int64_t z = row / d.ny, y = row - z * d.ny;
-        v = smp.at(z, y, x, st);
-      }
-    }
+    if (row < nrows && x < d.nx) v = vol[row * d.nx + x];
     tile[rr][lane] = v;
   }
 }
@@ -320,10 +288,10 @@ __device__ __forceinline__ bool consume_tile(const T* row, int lim, Op& op) {
   return false;
 }
 
-template <typename T, typename U, typename S, typename Op>
-__global__ void __launch_bounds__(kRays) k_rays_alongx(S smp, Op op0, U* __restrict__ out, int* status) {
+template <typename T, typename U, typename Op>
+__global__ void __launch_bounds__(kRays) k_rays_alongx(const T* __restrict__ vol, Dims d, Op op0, U* __restrict__ out,
+                                                       int* status) {
   __shared__ __align__(16) T tile[kRays][Pitch<T>::value];
-  const Dims d = smp.d;
   const int64_t nrows = d.nz * d.ny;
   const int64_t row0 = (int64_t)blockIdx.x * kRays;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -331,10 +299,9 @@ __global__ void __launch_bounds__(kRays) k_rays_alongx(S smp, Op op0, U* __restr
   const bool live = myrow < nrows;
   Op op = op0;
   op.init();
-  int st = 0;
   bool done = !live;
   for (int64_t x0 = 0; x0 < d.nx; x0 += kChunk) {
-    load_tile<T>(smp, tile, row0, nrows, x0, lane, warp, &st);
+    load_tile<T>(vol, d, tile, row0, nrows, x0, lane, warp);
     __syncthreads();
     if (!done) {
       if (x0 == 0) op.first(tile[tid][0]);
@@ -345,236 +312,85 @@ __global__ void __launch_bounds__(kRays) k_rays_alongx(S smp, Op op0, U* __restr
   }
   if (live) {
     U o;
-    if (op.result(&o)) out[myrow] = o; else st = B2V_ERR_RANGE;
+    if (op.result(&o)) out[myrow] = o; else *status = B2V_ERR_RANGE;
   }
-  if (st) *status = st;
 }
 
-// ---- rays along x, int16: rows staged by the TMA engine ---------------------------------------------
-// cp.async.bulk (1-D bulk tensor copy, global -> shared, completion counted on an mbarrier): every
-// thread asks the copy engine for the next 64-sample segment (128 B) of ITS ray and goes back to
-// the float32 recurrence; no thread spends issue slots on loads, and the segment after next is in
-// flight while the current one is consumed (two stages). Rows sit 144 B apart in shared memory, so
-// the 16-byte reads of eight consecutive threads fall into eight different bank groups.
-// Needs 16-byte aligned rows (nx % 8 == 0, aligned base); otherwise the lane-load kernels above run.
-constexpr int kTmaChunk = 64;                                  // samples per stage and ray
-constexpr int kTmaPitch = kTmaChunk * 2 + 16;                  // bytes between rows in shared memory
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  }
-}
-__device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-// the block's 128 rays through `op` (one per thread); returns false if a result does not fit
-template <typename U, typename Op>
-__device__ __forceinline__ void rays_alongx_tma(const int16_t* __restrict__ vol, Dims d, Op& op, bool call_first,
-                                                U* __restrict__ out, int* status) {
-  __shared__ __align__(16) unsigned char stage[2][kRays * kTmaPitch];
-  __shared__ __align__(8) uint64_t bar[2];
-  const int64_t nrows = d.nz * d.ny;
-  const int tid = threadIdx.x;
-  const int64_t myrow = (int64_t)blockIdx.x * kRays + tid;
-  const bool live = myrow < nrows;
-  const int nchunks = (int)ceil_div64(d.nx, kTmaChunk);
-  if (tid == 0) {
-    mbar_init(&bar[0], kRays);
-    mbar_init(&bar[1], kRays);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  const int16_t* row = vol + (live ? myrow : 0) * d.nx;
-  auto issue = [&](int k) {
-    const int b = k & 1;
-    const int64_t x0 = (int64_t)k * kTmaChunk;
-    const uint32_t bytes = live ? (uint32_t)(((d.nx - x0) < kTmaChunk ? (d.nx - x0) : kTmaChunk) * 2) : 0u;
-    mbar_arrive_expect_tx(&bar[b], bytes);
-    if (bytes) tma_load_1d(&stage[b][tid * kTmaPitch], row + x0, bytes, &bar[b]);
-  };
-  issue(0);
-  if (nchunks > 1) issue(1);
-  int issued = nchunks > 1 ? 2 : 1, waited = 0;
-  int st = 0;
-  bool done = !live;
-  for (int k = 0; k < nchunks; ++k) {
-    const int b = k & 1;
-    mbar_wait(&bar[b], (uint32_t)((k >> 1) & 1));
-    ++waited;
-    if (!done) {
-      const uint4* w = reinterpret_cast<const uint4*>(&stage[b][tid * kTmaPitch]);
-      const int lim = (int)((d.nx - (int64_t)k * kTmaChunk) < kTmaChunk ? (d.nx - (int64_t)k * kTmaChunk) : kTmaChunk);
-      if (k == 0 && call_first) op.first((int16_t)(w[0].x & 0xffffu));
-      for (int j = 0; j < kTmaChunk / 8 && !done; ++j) {
-        const uint4 q = w[j];
-        const uint32_t ww4[4] = {q.x, q.y, q.z, q.w};
-        const int base = j * 8;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          if (!done && base + e < lim) done = op.step((int16_t)((e & 1) ? (ww4[e >> 1] >> 16) : (ww4[e >> 1] & 0xffffu)));
-        }
-        if (base + 8 >= lim) break;
-      }
-    }
-    const bool all_done = __syncthreads_and(done);   // also: everyone has finished reading stage b
-    if (all_done) break;
-    if (k + 2 < nchunks) { issue(k + 2); ++issued; }
-  }
-  // a segment may still be in flight when the rays ended early: let it land before the block leaves
-  for (int k = waited; k < issued; ++k) mbar_wait(&bar[k & 1], (uint32_t)((k >> 1) & 1));
-  if (live) {
-    U o;
-    if (op.result(&o)) out[myrow] = o; else st = B2V_ERR_RANGE;
-  }
-  if (st) *status = st;
-}
-
-template <typename U, typename Op>
-__global__ void __launch_bounds__(kRays) k_rays_alongx_tma(const int16_t* __restrict__ vol, Dims d, Op op0,
-                                                           U* __restrict__ out, int* status) {
-  Op op = op0;
+// ---- rays along z over ONE Z shard (dist: MIDA / LMIP with rays that cross the shards) ------
+// The ray of pixel (y, x) starts from the state the previous shard left (or is started here),
+// walks this slab and leaves its state for the next shard; the last shard writes the pixel.
+// The per-ray operation order is that of the whole-volume walk, so the result is bit-exact.
+template <typename T, typename U, typename Op>
+__global__ void __launch_bounds__(128) k_rays_z_partial(const T* __restrict__ vol, Dims d, Op op, uint32_t* state,
+                                                        int first, int last, U* __restrict__ out, int* status) {
+  const int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t y = blockIdx.y;
+  if (x >= d.nx) return;
+  const int64_t plane = d.ny * d.nx, i = y * d.nx + x;
+  bool done = false;
   op.init();
-  rays_alongx_tma<U, Op>(vol, d, op, true, out, status);
-}
-
-// Measured at 1024^3, rays along x (tools/mida_axis2.py, two alternating runs on one H100 80GB HBM3 at
-// a 400 W power limit): MIDA full rays 2.42-2.43 ms (TMA rows) vs 2.36-2.46 ms (lane loads), LMIP
-// 0.13-0.19 vs 0.10-0.11 ms — 128-byte bulk copies per thread are too small for the copy engine to
-// beat 32-bit lane loads here, and the rays are bound by the recurrence, not by the loads. The lane-load kernels stay the default; b2v_proj_set_tma(1) (or B2V_TMA=1) selects this path.
-int g_proj_tma = -1;
-inline bool tma_rows_ok(const void* vol, const Dims& d) {
-  if (g_proj_tma < 0) g_proj_tma = getenv("B2V_TMA") != nullptr ? 1 : 0;
-  return g_proj_tma == 1 && d.nx % 8 == 0 && (reinterpret_cast<uintptr_t>(vol) & 15u) == 0;
+  if (first) op.first(vol[i]);
+  else op.load(state, i, plane, &done);
+  if (!done) done = walk_keepx<T>(vol, d, 0, y, x, d.nz, op);
+  op.store(state, i, plane, done);
+  if (last) {
+    U o;
+    if (op.result(&o)) out[i] = o; else *status = B2V_ERR_RANGE;
+  }
 }
 
 __global__ void k_status_init(int* status) { *status = 0; }
 
-template <typename T, typename U, typename S, typename Op>
-int launch_rays(S smp, int axis, Op op, U* out, int* status, cudaStream_t s) {
-  const Dims d = smp.d;
+// `what` names the projection in the error message.
+template <typename T, typename U, typename Op>
+int launch_rays(const T* vol, Dims d, int axis, Op op, U* out, int* status, cudaStream_t s, const char* what) {
   if (axis == 2) {
-    int64_t nrows = d.nz * d.ny;
-    if constexpr (S::kLinear && sizeof(T) == 2) {
-      if (tma_rows_ok(smp.vol, d)) {
-        k_rays_alongx_tma<U, Op><<<(unsigned)ceil_div64(nrows, kRays), kRays, 0, s>>>((const int16_t*)smp.vol, d, op, out,
-                                                                                     status);
-        return b2v_check_launch("k_rays_alongx_tma");
-      }
-    }
-    k_rays_alongx<T, U, S, Op><<<(unsigned)ceil_div64(nrows, kRays), kRays, 0, s>>>(smp, op, out, status);
+    k_rays_alongx<T, U, Op><<<(unsigned)ceil_div64(d.nz * d.ny, kRays), kRays, 0, s>>>(vol, d, op, out, status);
     return b2v_check_launch("k_rays_alongx");
   }
   int64_t nr = axis == 0 ? d.ny : d.nz;
-  B2V_REQUIRE(nr <= 65535, B2V_ERR_ARG, "projection: more than 65535 output rows");
+  B2V_REQUIRE(nr <= 65535, B2V_ERR_ARG, "%s: more than 65535 output rows", what);
   dim3 grid((unsigned)ceil_div64(d.nx, 128), (unsigned)nr);
-  k_rays_keepx<T, U, S, Op><<<grid, 128, 0, s>>>(smp, axis, op, out, status);
+  k_rays_keepx<T, U, Op><<<grid, 128, 0, s>>>(vol, d, axis, op, out, status);
   return b2v_check_launch("k_rays_keepx");
 }
 
-// MidaOp needs (min, range, 1/range) which live on the device: a tiny kernel finishes the
-// operator there instead of synchronising.
-template <typename T, typename U, typename S>
-__global__ void __launch_bounds__(128) k_mida_keepx(S smp, int axis, const float* __restrict__ mm, float wl, float ww,
-                                                    U* __restrict__ out, int* status);
-
-template <typename T, typename U>
-__device__ __forceinline__ MidaOp<T, U> make_mida(const float* mm, float wl, float ww) {
-  MidaOp<T, U> op;
-  op.img_min = mm[0];
-  op.range = __fsub_rn(mm[1], mm[0]);
-  op.inv = __fdiv_rn(1.0f, op.range);
-  op.wl = wl;
-  op.ww = ww;
-  return op;
+template <typename T, typename U, typename Op>
+int launch_z_partial(const T* vol, Dims d, Op op, uint32_t* state, int first, int last, U* out, int* status,
+                     cudaStream_t s) {
+  const dim3 grid((unsigned)ceil_div64(d.nx, 128), (unsigned)d.ny);
+  k_rays_z_partial<T, U, Op><<<grid, 128, 0, s>>>(vol, d, op, state, first, last, out, status);
+  return b2v_check_launch("k_rays_z_partial");
 }
 
-template <typename T, typename U, typename S>
-__global__ void __launch_bounds__(128) k_mida_keepx(S smp, int axis, const float* __restrict__ mm, float wl, float ww,
-                                                    U* __restrict__ out, int* status) {
-  const Dims d = smp.d;
-  const int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t r = blockIdx.y;
-  if (x >= d.nx) return;
-  const int64_t n_l = axis == 0 ? d.nz : d.ny;
-  MidaOp<T, U> op = make_mida<T, U>(mm, wl, ww);
-  op.init();
-  int st = 0;
-  walk_keepx<T>(smp, axis, r, x, n_l, op, &st);
-  U o;
-  if (op.result(&o)) out[r * d.nx + x] = o; else st = B2V_ERR_RANGE;
-  if (st) *status = st;
+// ---- dtype dispatch: launch(vol, out, op) with the typed pointers and the operator -----------
+// MIDA's (image, output) dtype pairs (mips_py.rs:161-202); wl and ww are taken as the image type
+// (mips_py.rs:174-175). mm is the device (min, max) pair.
+template <typename Launch>
+int dispatch_mida(const void* img, int dtype, void* out, int out_dtype, double wl, double ww, const float* mm,
+                  Launch&& launch) {
+  auto with = [&](auto t, auto u) {
+    using T = decltype(t);
+    using U = decltype(u);
+    return launch((const T*)img, (U*)out, MidaOp<T, U>{mm, (float)(T)wl, (float)(T)ww});
+  };
+  if (dtype == B2V_I16 && out_dtype == B2V_I16) return with(int16_t(), int16_t());
+  if (dtype == B2V_U8 && out_dtype == B2V_U8) return with(uint8_t(), uint8_t());
+  if (dtype == B2V_F64 && out_dtype == B2V_U8) return with(double(), uint8_t());
+  B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
 }
 
-template <typename T, typename U, typename S>
-__global__ void __launch_bounds__(kRays) k_mida_alongx(S smp, const float* __restrict__ mm, float wl, float ww,
-                                                       U* __restrict__ out, int* status) {
-  __shared__ __align__(16) T tile[kRays][Pitch<T>::value];
-  const Dims d = smp.d;
-  const int64_t nrows = d.nz * d.ny;
-  const int64_t row0 = (int64_t)blockIdx.x * kRays;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t myrow = row0 + tid;
-  const bool live = myrow < nrows;
-  MidaOp<T, U> op = make_mida<T, U>(mm, wl, ww);
-  op.init();
-  int st = 0;
-  bool done = !live;
-  for (int64_t x0 = 0; x0 < d.nx; x0 += kChunk) {
-    load_tile<T>(smp, tile, row0, nrows, x0, lane, warp, &st);
-    __syncthreads();
-    if (!done) {
-      int lim = (int)((d.nx - x0) < kChunk ? (d.nx - x0) : kChunk);
-      done = consume_tile<T>(tile[tid], lim, op);
-    }
-    if (__syncthreads_and(done)) break;
-  }
-  if (live) {
-    U o;
-    if (op.result(&o)) out[myrow] = o; else st = B2V_ERR_RANGE;
-  }
-  if (st) *status = st;
-}
-
-template <typename U>
-__global__ void __launch_bounds__(kRays) k_mida_alongx_tma(const int16_t* __restrict__ vol, Dims d,
-                                                           const float* __restrict__ mm, float wl, float ww,
-                                                           U* __restrict__ out, int* status) {
-  MidaOp<int16_t, U> op = make_mida<int16_t, U>(mm, wl, ww);
-  op.init();
-  rays_alongx_tma<U, MidaOp<int16_t, U>>(vol, d, op, false, out, status);
-}
-
-template <typename T, typename U, typename S>
-int launch_mida(S smp, int axis, const float* mm, float wl, float ww, U* out, int* status, cudaStream_t s) {
-  const Dims d = smp.d;
-  if (axis == 2) {
-    if constexpr (S::kLinear && sizeof(T) == 2) {
-      if (tma_rows_ok(smp.vol, d)) {
-        k_mida_alongx_tma<U><<<(unsigned)ceil_div64(d.nz * d.ny, kRays), kRays, 0, s>>>((const int16_t*)smp.vol, d, mm, wl,
-                                                                                      ww, out, status);
-        return b2v_check_launch("k_mida_alongx_tma");
-      }
-    }
-    k_mida_alongx<T, U, S><<<(unsigned)ceil_div64(d.nz * d.ny, kRays), kRays, 0, s>>>(smp, mm, wl, ww, out, status);
-    return b2v_check_launch("k_mida_alongx");
-  }
-  int64_t nr = axis == 0 ? d.ny : d.nz;
-  B2V_REQUIRE(nr <= 65535, B2V_ERR_ARG, "mida: more than 65535 output rows");
-  dim3 grid((unsigned)ceil_div64(d.nx, 128), (unsigned)nr);
-  k_mida_keepx<T, U, S><<<grid, 128, 0, s>>>(smp, axis, mm, wl, ww, out, status);
-  return b2v_check_launch("k_mida_keepx");
+// LMIP takes int16, uint8 or float64, the output of the same dtype, tmin and tmax as that dtype.
+template <typename Launch>
+int dispatch_lmip(const void* img, int dtype, void* out, double tmin, double tmax, Launch&& launch) {
+  auto with = [&](auto t) {
+    using T = decltype(t);
+    return launch((const T*)img, (T*)out, LmipOp<T>{(T)tmin, (T)tmax});
+  };
+  if (dtype == B2V_I16) return with(int16_t());
+  if (dtype == B2V_U8) return with(uint8_t());
+  if (dtype == B2V_F64) return with(double());
+  B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
 }
 
 int finish_status(int* status_dev, cudaStream_t s, const char* what) {
@@ -606,50 +422,7 @@ bool check_axis_dims(int64_t dz, int64_t dy, int64_t dx, int axis) {
   return dz > 0 && dy > 0 && dx > 0 && axis >= 0 && axis <= 2;
 }
 
-// ---- rays along z over ONE Z shard (dist: MIDA / LMIP with rays that cross the shards) ------
-// The ray of pixel (y, x) starts from the state the previous shard left (or is started here),
-// walks this slab and leaves its state for the next shard; the last shard writes the pixel.
-// The per-ray operation order is that of the whole-volume walk, so the result is bit-exact.
-template <typename T, typename U, typename Op>
-__device__ __forceinline__ void ray_z_partial(const PlainSampler<T>& smp, Op& op, uint32_t* state, int first, int last,
-                                              U* out, int* status) {
-  const Dims d = smp.d;
-  const int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t y = blockIdx.y;
-  if (x >= d.nx) return;
-  const int64_t plane = d.ny * d.nx, i = y * d.nx + x;
-  int st = 0;
-  bool done = false;
-  op.init();
-  if (first) op.first(smp.vol[i]);
-  else op.load(state, i, plane, &done);
-  if (!done) done = walk_keepx<T>(smp, 0, y, x, d.nz, op, &st);
-  op.store(state, i, plane, done);
-  if (last) {
-    U o;
-    if (op.result(&o)) out[i] = o; else st = B2V_ERR_RANGE;
-  }
-  if (st) *status = st;
-}
-
-template <typename T, typename U>
-__global__ void __launch_bounds__(128) k_mida_z_partial(PlainSampler<T> smp, const float* __restrict__ mm, float wl,
-                                                        float ww, uint32_t* state, int first, int last,
-                                                        U* __restrict__ out, int* status) {
-  MidaOp<T, U> op = make_mida<T, U>(mm, wl, ww);
-  ray_z_partial<T, U>(smp, op, state, first, last, out, status);
-}
-
-template <typename T>
-__global__ void __launch_bounds__(128) k_lmip_z_partial(PlainSampler<T> smp, LmipOp<T> op0, uint32_t* state, int first,
-                                                        int last, T* __restrict__ out, int* status) {
-  LmipOp<T> op = op0;
-  ray_z_partial<T, T>(smp, op, state, first, last, out, status);
-}
-
 }  // namespace
-
-extern "C" void b2v_proj_set_tma(int on) { g_proj_tma = on ? 1 : 0; }
 
 extern "C" int64_t b2v_proj_workspace_bytes(int64_t n) { return 256 + b2v_minmax_workspace_bytes(n); }
 
@@ -669,20 +442,9 @@ static int mida_impl(const void* img, int dtype, int64_t dz, int64_t dy, int64_t
   } else if ((rc = b2v_minmax_f32(img, dtype, dz * dy * dx, w.mm_f, w.minmax_ws, stream))) {
     return rc;
   }
-  if (dtype == B2V_I16 && out_dtype == B2V_I16) {
-    PlainSampler<int16_t> smp = {(const int16_t*)img, d};
-    rc = launch_mida<int16_t, int16_t>(smp, axis, w.mm_f, (float)(int16_t)wl, (float)(int16_t)ww, (int16_t*)out,
-                                       w.status, s);
-  } else if (dtype == B2V_U8 && out_dtype == B2V_U8) {
-    PlainSampler<uint8_t> smp = {(const uint8_t*)img, d};
-    rc = launch_mida<uint8_t, uint8_t>(smp, axis, w.mm_f, (float)(uint8_t)wl, (float)(uint8_t)ww, (uint8_t*)out,
-                                       w.status, s);
-  } else if (dtype == B2V_F64 && out_dtype == B2V_U8) {
-    PlainSampler<double> smp = {(const double*)img, d};
-    rc = launch_mida<double, uint8_t>(smp, axis, w.mm_f, (float)wl, (float)ww, (uint8_t*)out, w.status, s);
-  } else {
-    B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
-  }
+  rc = dispatch_mida(img, dtype, out, out_dtype, wl, ww, w.mm_f, [&](auto* vol, auto* o, auto op) {
+    return launch_rays(vol, d, axis, op, o, w.status, s, "mida");
+  });
   if (rc) return rc;
   return finish_status(w.status, s, "mida");
 }
@@ -709,25 +471,9 @@ extern "C" int b2v_lmip(const void* img, int dtype, int64_t dz, int64_t dy, int6
   int rc;
   k_status_init<<<1, 1, 0, s>>>(w.status);
   if ((rc = b2v_check_launch("k_status_init"))) return rc;
-  if (dtype == B2V_I16) {
-    PlainSampler<int16_t> smp = {(const int16_t*)img, d};
-    LmipOp<int16_t> op;
-    op.tmin = (int16_t)tmin; op.tmax = (int16_t)tmax;
-    rc = launch_rays<int16_t, int16_t>(smp, axis, op, (int16_t*)out, w.status, s);
-  } else if (dtype == B2V_U8) {
-    PlainSampler<uint8_t> smp = {(const uint8_t*)img, d};
-    LmipOp<uint8_t> op;
-    op.tmin = (uint8_t)tmin; op.tmax = (uint8_t)tmax;
-    rc = launch_rays<uint8_t, uint8_t>(smp, axis, op, (uint8_t*)out, w.status, s);
-  } else if (dtype == B2V_F64) {
-    PlainSampler<double> smp = {(const double*)img, d};
-    LmipOp<double> op;
-    op.tmin = tmin; op.tmax = tmax;
-    rc = launch_rays<double, double>(smp, axis, op, (double*)out, w.status, s);
-  } else {
-    B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
-  }
-  return rc;
+  return dispatch_lmip(img, dtype, out, tmin, tmax, [&](auto* vol, auto* o, auto op) {
+    return launch_rays(vol, d, axis, op, o, w.status, s, "projection");
+  });
 }
 
 // ---- the contour volume itself (mips.rs:238-242: tmp[z, y, x] = T(calc_fcm_intensity)) -------------
@@ -909,23 +655,10 @@ extern "C" int b2v_mida_z_partial(const void* img, int dtype, int64_t dz, int64_
   k_status_init<<<1, 1, 0, s>>>(w.status);
   if ((rc = b2v_check_launch("k_status_init"))) return rc;
   B2V_CUDA(cudaMemcpyAsync(w.mm_f, minmax_dev, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  const dim3 grid((unsigned)ceil_div64(dx, 128), (unsigned)dy);
-  if (dtype == B2V_I16 && out_dtype == B2V_I16) {
-    PlainSampler<int16_t> smp = {(const int16_t*)img, d};
-    k_mida_z_partial<int16_t, int16_t><<<grid, 128, 0, s>>>(smp, w.mm_f, (float)(int16_t)wl, (float)(int16_t)ww, state,
-                                                            first, last, (int16_t*)out, w.status);
-  } else if (dtype == B2V_U8 && out_dtype == B2V_U8) {
-    PlainSampler<uint8_t> smp = {(const uint8_t*)img, d};
-    k_mida_z_partial<uint8_t, uint8_t><<<grid, 128, 0, s>>>(smp, w.mm_f, (float)(uint8_t)wl, (float)(uint8_t)ww, state,
-                                                          first, last, (uint8_t*)out, w.status);
-  } else if (dtype == B2V_F64 && out_dtype == B2V_U8) {
-    PlainSampler<double> smp = {(const double*)img, d};
-    k_mida_z_partial<double, uint8_t><<<grid, 128, 0, s>>>(smp, w.mm_f, (float)wl, (float)ww, state, first, last,
-                                                         (uint8_t*)out, w.status);
-  } else {
-    B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
-  }
-  if ((rc = b2v_check_launch("k_mida_z_partial"))) return rc;
+  rc = dispatch_mida(img, dtype, out, out_dtype, wl, ww, w.mm_f, [&](auto* vol, auto* o, auto op) {
+    return launch_z_partial(vol, d, op, state, first, last, o, w.status, s);
+  });
+  if (rc) return rc;
   return finish_status(w.status, s, "mida_z_partial");
 }
 
@@ -941,24 +674,7 @@ extern "C" int b2v_lmip_z_partial(const void* img, int dtype, int64_t dz, int64_
   int rc;
   k_status_init<<<1, 1, 0, s>>>(w.status);
   if ((rc = b2v_check_launch("k_status_init"))) return rc;
-  const dim3 grid((unsigned)ceil_div64(dx, 128), (unsigned)dy);
-  if (dtype == B2V_I16) {
-    PlainSampler<int16_t> smp = {(const int16_t*)img, d};
-    LmipOp<int16_t> op;
-    op.tmin = (int16_t)tmin; op.tmax = (int16_t)tmax;
-    k_lmip_z_partial<int16_t><<<grid, 128, 0, s>>>(smp, op, state, first, last, (int16_t*)out, w.status);
-  } else if (dtype == B2V_U8) {
-    PlainSampler<uint8_t> smp = {(const uint8_t*)img, d};
-    LmipOp<uint8_t> op;
-    op.tmin = (uint8_t)tmin; op.tmax = (uint8_t)tmax;
-    k_lmip_z_partial<uint8_t><<<grid, 128, 0, s>>>(smp, op, state, first, last, (uint8_t*)out, w.status);
-  } else if (dtype == B2V_F64) {
-    PlainSampler<double> smp = {(const double*)img, d};
-    LmipOp<double> op;
-    op.tmin = tmin; op.tmax = tmax;
-    k_lmip_z_partial<double><<<grid, 128, 0, s>>>(smp, op, state, first, last, (double*)out, w.status);
-  } else {
-    B2V_REQUIRE(false, B2V_ERR_ARG, "Invalid image or output type");
-  }
-  return b2v_check_launch("k_lmip_z_partial");
+  return dispatch_lmip(img, dtype, out, tmin, tmax, [&](auto* vol, auto* o, auto op) {
+    return launch_z_partial(vol, d, op, state, first, last, o, w.status, s);
+  });
 }
