@@ -364,6 +364,24 @@ int b2v_voronoi_borders(const int32_t* owners, int64_t dz, int64_t dy, int64_t d
 int b2v_image_normalize_f32_i16(const float* in, int64_t n, float imin, float imax, float span, float min_f,
                                 int16_t fill, int16_t* out, void* stream);
 
+/* ---- binary morphology ---------------------------------------------------------------------------
+ * b2v_binary_morphology: scipy.ndimage.binary_erosion(border_value=True) / binary_dilation(border_value=False)
+ *   with the Euclidean footprint {d : |d|^2 <= radius^2}: skimage's disk(radius) on every z-slice alone
+ *   (planar != 0) or ball(radius) on the volume (planar == 0), as the mask-morphology plugin applies them
+ *   (plugins/mask_morphology/gui.py:98-175). in: dense uint8 [dz][dy][dx]; a voxel is set where in > threshold.
+ *   out: dense uint8 [dz][dy][dx] (not aliasing in), set_value where the result is set, else 0. counts: device
+ *   int64[2], overwritten with the set voxels of the input and of the result. radius 0 (the identity) .. 15;
+ *   anything else, or an op other than B2V_MORPH_ERODE / B2V_MORPH_DILATE, is B2V_ERR_ARG. workspace:
+ *   b2v_binary_morphology_workspace_bytes (planar: 0; volumetric: one byte per voxel with rows padded to a
+ *   multiple of 4). Exact integer arithmetic: the bounded squared distance to the nearest source voxel is
+ *   taken one axis at a time. Algorithmic bytes: planar 2 B per voxel (in read, out written); volumetric 4 B
+ *   (in, the workspace written and read, out). */
+#define B2V_MORPH_ERODE 0
+#define B2V_MORPH_DILATE 1
+int64_t b2v_binary_morphology_workspace_bytes(int64_t dz, int64_t dy, int64_t dx, int planar);
+int b2v_binary_morphology(const uint8_t* in, int64_t dz, int64_t dy, int64_t dx, uint8_t threshold, int op, int radius,
+                          int planar, uint8_t set_value, uint8_t* out, int64_t* counts, void* workspace, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,
