@@ -331,6 +331,30 @@ int64_t b2v_zoom_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order);
 int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int64_t ny, int64_t nx, int64_t out_nz, int64_t out_ny,
              int64_t out_nx, int order, int mode, double cval, void* out, int out_dtype, void* workspace, void* stream);
 
+/* b2v_shift: scipy.ndimage.shift(input, shift, output, order, mode, cval) with prefilter=True, the call behind
+ * imagedata_utils.FixGantryTilt (imagedata_utils.py:28, :143-154). Arguments as b2v_zoom's, with the output of the
+ * input's shape (out != in) and shift: host array of ndim float64 values in axis order. Output index o samples
+ * input coordinate o - shift per axis. mode B2V_ZOOM_CONSTANT writes cval where a coordinate is below 0 or above
+ * n - 1 (strict on both sides); B2V_ZOOM_MIRROR folds it as SciPy does. Workspace and algorithmic bytes as
+ * b2v_zoom's at a factor of 1 (b2v_shift_workspace_bytes: 8 B per voxel for orders 2 and 3, else 0). Bit-exact. */
+int64_t b2v_shift_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order);
+int b2v_shift(const void* in, int in_dtype, int ndim, int64_t nz, int64_t ny, int64_t nx, const double* shift,
+              int order, int mode, double cval, void* out, int out_dtype, void* workspace, void* stream);
+
+/* b2v_gantry_tilt: imagedata_utils.FixGantryTilt in place on a dense int16 [nz][ny][nx] device volume: slice n is
+ * replaced by scipy.ndimage.shift(slice n, shifts[2n : 2n + 2], order=3, mode='constant', cval=matrix.min()), the
+ * minimum taken over the volume as the sequential loop leaves it (shifted slices 0..n-1, original slices n..).
+ * shifts: host array of nz (y, x) pairs, computed by the caller in the reference's float64 order. The slices are
+ * interpolated together; the cvals come from a scan over per-slice minima (see zoom.cu). cvals: optional device
+ * array of nz int16 that receives each slice's cval (NULL: not written). slab: slices per prefilter pass (0: as
+ * many as fit 1 GiB of float64), so b2v_gantry_tilt_workspace_bytes is 8 B per voxel of one slab plus 32 B per
+ * slice, not of the volume. Algorithmic bytes: 2 B per voxel read for the original slice minima; then per slab
+ * 2 B + 3 x 8 B read and 2 x 8 B written by the y pass, 3 x 8 B read and 2 x 8 B written by the x pass, and the
+ * gather's ~8 B read and 2 B written per voxel; the fill writes 2 B per out-of-range voxel. Bit-exact. */
+int64_t b2v_gantry_tilt_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int64_t slab);
+int b2v_gantry_tilt(int16_t* vol, int64_t nz, int64_t ny, int64_t nx, const double* shifts, int64_t slab,
+                    void* workspace, int16_t* cvals, void* stream);
+
 /* ---- porous scaffolds: Voronoi ---------------------------------------------------------------------
  * The "Voronoi" scaffolds of the porous-creation plugin (plugins/porous_creation/schwarzp.py:37-84).
  * b2v_jump_flooding: invesalius_rs.jump_flooding(distance_map, map_owners, sites, normalize)

@@ -106,6 +106,10 @@ PROTOTYPES = {
     "b2v_masked_moments": (cint, [vp, cint, i64, i64, i64, vp, cint, cint, vp, vp, vp, vp]),
     "b2v_zoom_workspace_bytes": (i64, [i64, i64, i64, cint]),
     "b2v_zoom": (cint, [vp, cint, cint, i64, i64, i64, i64, i64, i64, cint, cint, dbl, vp, cint, vp, vp]),
+    "b2v_shift_workspace_bytes": (i64, [i64, i64, i64, cint]),
+    "b2v_shift": (cint, [vp, cint, cint, i64, i64, i64, vp, cint, cint, dbl, vp, cint, vp, vp]),
+    "b2v_gantry_tilt_workspace_bytes": (i64, [i64, i64, i64, i64]),
+    "b2v_gantry_tilt": (cint, [vp, i64, i64, i64, vp, i64, vp, vp, vp]),
     "b2v_jump_flooding_workspace_bytes": (i64, [i64, i64, i64, i64]),
     "b2v_jump_flooding": (cint, [vp, vp, i64, i64, i64, vp, i64, cint, vp, vp]),
     "b2v_voronoi_borders": (cint, [vp, i64, i64, i64, cint, vp, vp]),

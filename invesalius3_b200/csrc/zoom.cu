@@ -17,8 +17,31 @@
 //                            by the axis weights in axis order. In 'constant' mode a coordinate past n - 1 (the last
 //                            sample's o * step can round just above it) writes cval, as SciPy does. Integer outputs
 //                            round half away from zero and clip to the type's range.
+//
+// scipy.ndimage.shift(input, shift, output, order <= 3, mode) with prefilter=True shares SciPy's routine with zoom
+// (zoom_shift): the same prefilter, weights, folding, tap order and rounding, with coordinate o - shift per axis.
+// Shift coordinates can be negative, so 'constant' mode writes cval on both sides (cc < 0 or cc > n - 1) and
+// 'mirror' folds negative coordinates as SciPy's map_coordinate does. Zoom coordinates are never negative, so
+// those branches leave zoom results unchanged.
+//   k_shift_gather<T, ORDER> one thread per output voxel, one slice per grid row: SciPy's 3-D sum for volumes, its
+//                            2-D sum for a stack of slices, each slice with its own (y, x) shift.
+//
+// imagedata_utils.FixGantryTilt (imagedata_utils.py:143-154) shifts slice n of an int16 volume in place along y at
+// order 3 with cval = matrix.min() of the partly shifted volume. b2v_gantry_tilt evaluates it without the
+// sequential loop: cval[n] = min(min of original slices n.., min of shifted slices ..n-1), where a shifted slice's
+// minimum is the minimum of its in-range outputs (independent of cval), lowered to cval[k] if it has out-of-range
+// outputs (a property of its shift alone). So every slice is interpolated at once, then a scan over nz scalars
+// gives the cvals, then the out-of-range outputs are filled.
+//   k_slice_min_i16          per-slice minimum of the original volume, before any slice is overwritten
+//   (prefilter, slab by slab) y then x passes over a slab of slices into a float64 workspace of the slab's size
+//   k_shift_gather<double,3> writes the in-range outputs in place, records per-slice in-range minima (warp
+//                            min-reduce, one int atomicMin per warp: order-independent) and out-of-range flags
+//   k_tilt_cval_chain        the scan over nz scalars (one thread)
+//   k_tilt_fill              writes each slice's cval into its out-of-range outputs
+#include <limits.h>
 #include <math.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "b2v_common.cuh"
@@ -190,19 +213,25 @@ __device__ __forceinline__ int64_t fold_mirror(int64_t i, int64_t n) {
   return m >= n ? p - m : m;
 }
 
-// Coordinate, weights and folded tap indices of output index o along one axis; false where 'constant' mode
-// writes cval.
+// 'constant' mode writes cval at a coordinate outside [0, n - 1] (SciPy's test is strict on both sides)
+__device__ __forceinline__ bool outside_axis(double cc, int64_t n) { return cc < 0.0 || cc > (double)(n - 1); }
+
+// Weights and folded tap indices at coordinate cc of an axis of n_in samples; false where 'constant' mode writes
+// cval.
 template <int ORDER>
-__device__ __forceinline__ bool axis_taps(const Axis& A, int64_t o, bool mirror, double* w, int64_t* idx) {
-  double cc = (double)o * A.step;
-  if (cc > (double)(A.n_in - 1)) {
+__device__ __forceinline__ bool taps_at(double cc, int64_t n_in, bool mirror, double* w, int64_t* idx) {
+  if (outside_axis(cc, n_in)) {
     if (!mirror) return false;
-    if (A.n_in == 1) {
+    if (n_in == 1) {
       cc = 0.0;
+    } else if (cc < 0.0) {   // SciPy's map_coordinate, in its operation order
+      const int64_t p = 2 * n_in - 2;
+      cc = (double)(p * (int64_t)(-cc / (double)p)) + cc;
+      cc = cc <= (double)(1 - n_in) ? cc + (double)p : -cc;
     } else {
-      const double p = (double)(2 * A.n_in - 2);
+      const double p = (double)(2 * n_in - 2);
       cc -= p * (double)(int64_t)(cc / p);
-      if (cc >= (double)A.n_in) cc = p - cc;
+      if (cc >= (double)n_in) cc = p - cc;
     }
   }
   const double f = (ORDER & 1) ? floor(cc) : floor(cc + 0.5);
@@ -225,19 +254,34 @@ __device__ __forceinline__ bool axis_taps(const Axis& A, int64_t o, bool mirror,
   w[ORDER] = last;
   const int64_t start = (int64_t)f - ORDER / 2;
 #pragma unroll
-  for (int k = 0; k <= ORDER; ++k) idx[k] = fold_mirror(start + k, A.n_in);
+  for (int k = 0; k <= ORDER; ++k) idx[k] = fold_mirror(start + k, n_in);
   return true;
 }
 
+// Coordinate, weights and folded tap indices of output index o along one zoomed axis
+template <int ORDER>
+__device__ __forceinline__ bool axis_taps(const Axis& A, int64_t o, bool mirror, double* w, int64_t* idx) {
+  return taps_at<ORDER>((double)o * A.step, A.n_in, mirror, w, idx);
+}
+
 template <typename T>
-__device__ __forceinline__ void store_rounded(void* out, int64_t i, double t) {
+__device__ __forceinline__ T round_clip(double t) {
   if (t > 0.0) t += 0.5;
   else t = (T)-1 < (T)0 ? t - 0.5 : 0.0;   // unsigned: everything up to 0 becomes 0
   const double lo = (double)((T)-1 < (T)0 ? (T)(1 << (8 * sizeof(T) - 1)) : (T)0);
   const double hi = (double)((T)-1 < (T)0 ? (T)((1 << (8 * sizeof(T) - 1)) - 1) : (T)-1);
   t = t > hi ? hi : t;
   t = t < lo ? lo : t;
-  ((T*)out)[i] = (T)t;   // truncation
+  return (T)t;   // truncation
+}
+
+__device__ __forceinline__ void store_out(int out_dtype, void* out, int64_t i, double t) {
+  switch (out_dtype) {
+    case B2V_I16: ((int16_t*)out)[i] = round_clip<int16_t>(t); break;
+    case B2V_U8: ((uint8_t*)out)[i] = round_clip<uint8_t>(t); break;
+    case B2V_F32: ((float*)out)[i] = (float)t; break;
+    default: ((double*)out)[i] = t; break;
+  }
 }
 
 template <typename T, int ORDER>
@@ -279,13 +323,146 @@ __global__ void __launch_bounds__(256) k_zoom_gather(const T* __restrict__ src, 
         }
       }
     }
-    switch (P.out_dtype) {
-      case B2V_I16: store_rounded<int16_t>(out, i, t); break;
-      case B2V_U8: store_rounded<uint8_t>(out, i, t); break;
-      case B2V_F32: ((float*)out)[i] = (float)t; break;
-      default: ((double*)out)[i] = t; break;
+    store_out(P.out_dtype, out, i, t);
+  }
+}
+
+// ---- shift --------------------------------------------------------------------------------------------
+struct ShiftParams {
+  int64_t nz, ny, nx;          // input = output shape; a stack of 2-D slices when rank3 is 0
+  double shift[3];             // z, y, x: output index o samples input coordinate o - shift
+  const double* slice_shift;   // stack of slices: per-slice (y, x) shifts on the device, or null (shift[1], shift[2])
+  int rank3, mirror, out_dtype;
+  double cval;
+  // Stack of slices with int16 output (gantry tilt): out-of-range outputs are left unwritten; slice_min receives
+  // the per-slice minimum of the in-range outputs and slice_out is set where a slice has an out-of-range output.
+  int* slice_min;
+  int* slice_out;
+};
+
+template <typename T, int ORDER>
+__global__ void __launch_bounds__(256) k_shift_gather(const T* __restrict__ src, ShiftParams P, void* out) {
+  const int64_t area = P.ny * P.nx;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int kz_taps = P.rank3 ? ORDER + 1 : 1;
+  for (int64_t oz = blockIdx.y; oz < P.nz; oz += gridDim.y) {   // uniform across the block
+    double wz[ORDER + 1];
+    int64_t iz[ORDER + 1];
+    bool z_inside = true;
+    double sy = P.shift[1], sx = P.shift[2];
+    const T* plane = src;
+    iz[0] = 0;
+    if (P.rank3) {
+      z_inside = taps_at<ORDER>((double)oz - P.shift[0], P.nz, P.mirror, wz, iz);
+    } else {
+      plane = src + oz * area;
+      if (P.slice_shift) {
+        sy = P.slice_shift[2 * oz];
+        sx = P.slice_shift[2 * oz + 1];
+      }
+    }
+    int vmin = INT_MAX;
+    bool any_out = false;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < area; i += stride) {
+      const int64_t ox = i % P.nx, oy = i / P.nx, o = oz * area + i;
+      double wy[ORDER + 1], wx[ORDER + 1];
+      int64_t iy[ORDER + 1], ix[ORDER + 1];
+      const bool inside = z_inside && taps_at<ORDER>((double)oy - sy, P.ny, P.mirror, wy, iy) &&
+                          taps_at<ORDER>((double)ox - sx, P.nx, P.mirror, wx, ix);
+      if (!inside) {
+        if (P.slice_min) any_out = true;
+        else store_out(P.out_dtype, out, o, P.cval);
+        continue;
+      }
+      double t = 0.0;
+#pragma unroll
+      for (int a = 0; a <= ORDER; ++a) {
+        if (a == kz_taps) break;
+        const T* pz = plane + iz[a] * area;
+#pragma unroll
+        for (int b = 0; b <= ORDER; ++b) {
+          const T* py = pz + iy[b] * P.nx;
+#pragma unroll
+          for (int c = 0; c <= ORDER; ++c) {
+            double v = to_f64(py[ix[c]]);
+            if (ORDER > 0) {
+              if (P.rank3) v *= wz[a];
+              v *= wy[b];
+              v *= wx[c];
+            }
+            t += v;
+          }
+        }
+      }
+      if (P.slice_min) {
+        const int16_t r = round_clip<int16_t>(t);
+        ((int16_t*)out)[o] = r;
+        vmin = min(vmin, (int)r);
+      } else {
+        store_out(P.out_dtype, out, o, t);
+      }
+    }
+    if (P.slice_min) {
+      vmin = __reduce_min_sync(0xffffffffu, vmin);
+      any_out = __any_sync(0xffffffffu, any_out);
+      if ((threadIdx.x & 31) == 0) {
+        atomicMin(P.slice_min + oz, vmin);
+        if (any_out) P.slice_out[oz] = 1;
+      }
     }
   }
+}
+
+// per-slice minimum of a [nz][area] int16 volume into slice_min (initialised above every int16)
+__global__ void __launch_bounds__(256) k_slice_min_i16(const int16_t* __restrict__ vol, int64_t nz, int64_t area,
+                                                       int* slice_min) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t oz = blockIdx.y; oz < nz; oz += gridDim.y) {
+    int vmin = INT_MAX;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < area; i += stride)
+      vmin = min(vmin, (int)vol[oz * area + i]);
+    vmin = __reduce_min_sync(0xffffffffu, vmin);
+    if ((threadIdx.x & 31) == 0) atomicMin(slice_min + oz, vmin);
+  }
+}
+
+// cval[n] = min(min of original slices n.., min of shifted slices ..n-1), where shifted slice k's minimum is its
+// in-range minimum, lowered to cval[k] if it has out-of-range outputs. One thread: nz scalars.
+__global__ void k_tilt_cval_chain(int64_t nz, const int* orig_min, const int* inrange_min, const int* slice_out,
+                                  int* cval, int16_t* cval_out) {
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  int suffix = INT_MAX;
+  for (int64_t n = nz - 1; n >= 0; --n) {
+    suffix = min(suffix, orig_min[n]);
+    cval[n] = suffix;
+  }
+  int shifted = INT_MAX;
+  for (int64_t n = 0; n < nz; ++n) {
+    const int c = min(cval[n], shifted);
+    cval[n] = c;
+    if (cval_out) cval_out[n] = (int16_t)c;
+    shifted = min(shifted, slice_out[n] ? min(inrange_min[n], c) : inrange_min[n]);
+  }
+}
+
+// writes cval[z] into the outputs of slice z whose coordinate is outside the input (the gather's test)
+__global__ void __launch_bounds__(256) k_tilt_fill(int16_t* vol, int64_t nz, int64_t ny, int64_t nx,
+                                                   const double* slice_shift, const int* slice_out, const int* cval) {
+  const int64_t area = ny * nx, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t oz = blockIdx.y; oz < nz; oz += gridDim.y) {
+    if (!slice_out[oz]) continue;
+    const double sy = slice_shift[2 * oz], sx = slice_shift[2 * oz + 1];
+    const int16_t c = (int16_t)cval[oz];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < area; i += stride) {
+      const int64_t ox = i % nx, oy = i / nx;
+      if (outside_axis((double)oy - sy, ny) || outside_axis((double)ox - sx, nx)) vol[oz * area + i] = c;
+    }
+  }
+}
+
+// one grid row per slice (grid-stride beyond 65535 slices), blocks across the slice
+dim3 slice_grid(int64_t nz, int64_t area) {
+  return dim3((unsigned)std::min<int64_t>(ceil_div64(area, 256), 1024), (unsigned)std::min<int64_t>(nz, 65535));
 }
 
 int dtype_size(int dtype) {
@@ -306,12 +483,39 @@ Pole make_pole(int order, int64_t n) {
   return P;
 }
 
+// first prefilter pass: input dtype -> float64 along lines of length n, stride `inner`
 template <typename T>
-int prefilter_first(const void* in, double* ws, int64_t n, int64_t inner, int order, cudaStream_t s) {
-  const int64_t nlines = inner;
+int prefilter_first(const void* in, double* ws, int64_t n, int64_t inner, int64_t nlines, int order, cudaStream_t s) {
   k_prefilter_strided<T><<<(unsigned)ceil_div64(nlines, 256), 256, 0, s>>>((const T*)in, ws, n, inner, nlines,
                                                                            make_pole(order, n));
   return b2v_check_launch("k_prefilter_strided");
+}
+
+int prefilter_rows(double* ws, int64_t nx, int64_t nrows, int order, cudaStream_t s) {
+  if (nx == 1) return B2V_OK;
+  k_prefilter_rows<<<(unsigned)ceil_div64(nrows, 32 * kRowWarps), 32 * kRowWarps, 0, s>>>(ws, nx, nrows,
+                                                                                          make_pole(order, nx));
+  return b2v_check_launch("k_prefilter_rows");
+}
+
+// spline_filter(in, order, float64) of a [nz][ny][nx] volume into ws, axes z, y, x (nz = 1: a 2-D image)
+int prefilter_volume(const void* in, int in_dtype, int64_t nz, int64_t ny, int64_t nx, int order, double* ws,
+                     cudaStream_t s) {
+  int rc;
+  switch (in_dtype) {   // z pass: input dtype -> float64
+    case B2V_I16: rc = prefilter_first<int16_t>(in, ws, nz, ny * nx, ny * nx, order, s); break;
+    case B2V_U8: rc = prefilter_first<uint8_t>(in, ws, nz, ny * nx, ny * nx, order, s); break;
+    case B2V_F32: rc = prefilter_first<float>(in, ws, nz, ny * nx, ny * nx, order, s); break;
+    default: rc = prefilter_first<double>(in, ws, nz, ny * nx, ny * nx, order, s); break;
+  }
+  if (rc) return rc;
+  if (ny > 1) {
+    const int64_t nlines = nz * nx;
+    k_prefilter_strided<double><<<(unsigned)ceil_div64(nlines, 256), 256, 0, s>>>(ws, ws, ny, nx, nlines,
+                                                                                 make_pole(order, ny));
+    if ((rc = b2v_check_launch("k_prefilter_strided"))) return rc;
+  }
+  return prefilter_rows(ws, nx, nz * ny, order, s);
 }
 
 template <typename T, int ORDER>
@@ -332,6 +536,28 @@ int gather_order(const void* src, int order, const GatherParams& P, void* out, c
     if (order == 3) return gather_launch<T, 3>(src, P, out, s);
   }
   return order == 0 ? gather_launch<T, 0>(src, P, out, s) : gather_launch<T, 1>(src, P, out, s);
+}
+
+template <typename T, int ORDER>
+int shift_launch(const void* src, const ShiftParams& P, void* out, cudaStream_t s) {
+  k_shift_gather<T, ORDER><<<slice_grid(P.nz, P.ny * P.nx), 256, 0, s>>>((const T*)src, P, out);
+  return b2v_check_launch("k_shift_gather");
+}
+
+template <typename T>
+int shift_order(const void* src, int order, const ShiftParams& P, void* out, cudaStream_t s) {
+  if constexpr (std::is_same<T, double>::value) {
+    if (order == 2) return shift_launch<T, 2>(src, P, out, s);
+    if (order == 3) return shift_launch<T, 3>(src, P, out, s);
+  }
+  return order == 0 ? shift_launch<T, 0>(src, P, out, s) : shift_launch<T, 1>(src, P, out, s);
+}
+
+constexpr int64_t kTiltSlabBytes = int64_t(1) << 30;   // default float64 workspace of the gantry-tilt slab
+
+int64_t tilt_slab(int64_t nz, int64_t ny, int64_t nx, int64_t slab) {
+  if (slab <= 0) slab = std::max<int64_t>(1, kTiltSlabBytes / (ny * nx * (int64_t)sizeof(double)));
+  return std::min(slab, nz);
 }
 
 }  // namespace
@@ -360,28 +586,9 @@ extern "C" int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int6
   const void* src = in;
   int src_dtype = in_dtype;
   if (order >= 2) {
-    double* ws = (double*)workspace;
-    int rc;
-    switch (in_dtype) {   // z pass: input dtype -> float64
-      case B2V_I16: rc = prefilter_first<int16_t>(in, ws, nz, ny * nx, order, s); break;
-      case B2V_U8: rc = prefilter_first<uint8_t>(in, ws, nz, ny * nx, order, s); break;
-      case B2V_F32: rc = prefilter_first<float>(in, ws, nz, ny * nx, order, s); break;
-      default: rc = prefilter_first<double>(in, ws, nz, ny * nx, order, s); break;
-    }
+    const int rc = prefilter_volume(in, in_dtype, nz, ny, nx, order, (double*)workspace, s);
     if (rc) return rc;
-    if (ny > 1) {
-      const int64_t nlines = nz * nx;
-      k_prefilter_strided<double><<<(unsigned)ceil_div64(nlines, 256), 256, 0, s>>>(ws, ws, ny, nx, nlines,
-                                                                                   make_pole(order, ny));
-      if ((rc = b2v_check_launch("k_prefilter_strided"))) return rc;
-    }
-    if (nx > 1) {
-      const int64_t nrows = nz * ny;
-      k_prefilter_rows<<<(unsigned)ceil_div64(nrows, 32 * kRowWarps), 32 * kRowWarps, 0, s>>>(ws, nx, nrows,
-                                                                                              make_pole(order, nx));
-      if ((rc = b2v_check_launch("k_prefilter_rows"))) return rc;
-    }
-    src = ws;
+    src = workspace;
     src_dtype = B2V_F64;
   }
 
@@ -403,3 +610,103 @@ extern "C" int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int6
     default: return gather_order<double>(src, order, P, out, s);
   }
 }
+
+extern "C" int64_t b2v_shift_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order) {
+  return b2v_zoom_workspace_bytes(nz, ny, nx, order);
+}
+
+extern "C" int b2v_shift(const void* in, int in_dtype, int ndim, int64_t nz, int64_t ny, int64_t nx,
+                         const double* shift, int order, int mode, double cval, void* out, int out_dtype,
+                         void* workspace, void* stream) {
+  B2V_REQUIRE(dtype_size(in_dtype) && dtype_size(out_dtype), B2V_ERR_ARG, "shift: bad dtype code (%d, %d)",
+              in_dtype, out_dtype);
+  B2V_REQUIRE(order >= 0 && order <= 3, B2V_ERR_ARG, "shift: spline order %d not built (0-3)", order);
+  B2V_REQUIRE(mode == B2V_ZOOM_CONSTANT || mode == B2V_ZOOM_MIRROR, B2V_ERR_ARG, "shift: bad mode %d", mode);
+  B2V_REQUIRE(ndim == 2 || ndim == 3, B2V_ERR_ARG, "shift: ndim must be 2 or 3");
+  B2V_REQUIRE(ndim == 3 || nz == 1, B2V_ERR_ARG, "shift: a 2-D shift takes nz = 1");
+  B2V_REQUIRE(nz >= 0 && ny >= 0 && nx >= 0, B2V_ERR_ARG, "shift: negative size");
+  if (nz * ny * nx == 0) return B2V_OK;
+  B2V_REQUIRE(in && out && shift, B2V_ERR_ARG, "shift: null pointer");
+  B2V_REQUIRE(in != out, B2V_ERR_ARG, "shift: the output must not be the input");
+  B2V_REQUIRE(order < 2 || workspace, B2V_ERR_ARG, "shift: orders 2 and 3 need the workspace");
+  cudaStream_t s = (cudaStream_t)stream;
+
+  const void* src = in;
+  int src_dtype = in_dtype;
+  if (order >= 2) {
+    const int rc = prefilter_volume(in, in_dtype, nz, ny, nx, order, (double*)workspace, s);
+    if (rc) return rc;
+    src = workspace;
+    src_dtype = B2V_F64;
+  }
+
+  ShiftParams P = {};
+  P.nz = nz;
+  P.ny = ny;
+  P.nx = nx;
+  P.shift[0] = ndim == 3 ? shift[0] : 0.0;
+  P.shift[1] = shift[ndim - 2];
+  P.shift[2] = shift[ndim - 1];
+  P.rank3 = ndim == 3;
+  P.mirror = mode == B2V_ZOOM_MIRROR;
+  P.out_dtype = out_dtype;
+  P.cval = cval;
+  switch (src_dtype) {
+    case B2V_I16: return shift_order<int16_t>(src, order, P, out, s);
+    case B2V_U8: return shift_order<uint8_t>(src, order, P, out, s);
+    case B2V_F32: return shift_order<float>(src, order, P, out, s);
+    default: return shift_order<double>(src, order, P, out, s);
+  }
+}
+
+// workspace: [slab][ny][nx] float64 coefficients, nz (y, x) shifts, then four int arrays of nz
+extern "C" int64_t b2v_gantry_tilt_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int64_t slab) {
+  if (nz <= 0 || ny <= 0 || nx <= 0) return 0;
+  return tilt_slab(nz, ny, nx, slab) * ny * nx * (int64_t)sizeof(double) + nz * 2 * (int64_t)sizeof(double) +
+         nz * 4 * (int64_t)sizeof(int);
+}
+
+extern "C" int b2v_gantry_tilt(int16_t* vol, int64_t nz, int64_t ny, int64_t nx, const double* shifts, int64_t slab,
+                               void* workspace, int16_t* cvals, void* stream) {
+  B2V_REQUIRE(nz >= 0 && ny >= 0 && nx >= 0, B2V_ERR_ARG, "gantry_tilt: negative size");
+  if (nz * ny * nx == 0) return B2V_OK;
+  B2V_REQUIRE(vol && shifts && workspace, B2V_ERR_ARG, "gantry_tilt: null pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t area = ny * nx;
+  slab = tilt_slab(nz, ny, nx, slab);
+  double* ws = (double*)workspace;
+  double* d_shift = ws + slab * area;
+  int* orig_min = (int*)(d_shift + 2 * nz);
+  int* inrange_min = orig_min + nz;
+  int* slice_out = inrange_min + nz;
+  int* cval = slice_out + nz;
+
+  cudaError_t e = cudaMemcpyAsync(d_shift, shifts, nz * 2 * sizeof(double), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemsetAsync(orig_min, 0x7f, nz * 2 * sizeof(int), s);   // above every int16
+  if (e == cudaSuccess) e = cudaMemsetAsync(slice_out, 0, nz * sizeof(int), s);
+  B2V_REQUIRE(e == cudaSuccess, B2V_ERR_CUDA, "gantry_tilt: %s", cudaGetErrorString(e));
+  int rc;
+  k_slice_min_i16<<<slice_grid(nz, area), 256, 0, s>>>(vol, nz, area, orig_min);
+  if ((rc = b2v_check_launch("k_slice_min_i16"))) return rc;
+
+  ShiftParams P = {};
+  P.ny = ny;
+  P.nx = nx;
+  P.out_dtype = B2V_I16;
+  for (int64_t z0 = 0; z0 < nz; z0 += slab) {
+    const int64_t n = std::min(slab, nz - z0);
+    int16_t* sv = vol + z0 * area;   // the slab's slices are read by the prefilter before the gather overwrites them
+    if ((rc = prefilter_first<int16_t>(sv, ws, ny, nx, n * nx, 3, s))) return rc;
+    if ((rc = prefilter_rows(ws, nx, n * ny, 3, s))) return rc;
+    P.nz = n;
+    P.slice_shift = d_shift + 2 * z0;
+    P.slice_min = inrange_min + z0;
+    P.slice_out = slice_out + z0;
+    if ((rc = shift_launch<double, 3>(ws, P, sv, s))) return rc;
+  }
+  k_tilt_cval_chain<<<1, 32, 0, s>>>(nz, orig_min, inrange_min, slice_out, cval, cvals);
+  if ((rc = b2v_check_launch("k_tilt_cval_chain"))) return rc;
+  k_tilt_fill<<<slice_grid(nz, area), 256, 0, s>>>(vol, nz, ny, nx, d_shift, slice_out, cval);
+  return b2v_check_launch("k_tilt_fill");
+}
+
