@@ -221,6 +221,34 @@ int b2v_sharpen_i16(const int16_t* img, const double* blurred, int64_t n, double
 int b2v_sobel_magnitude(double* sx_inout, const double* sy, const double* sz, int64_t n, void* stream);
 int b2v_rescale_cast_i16(const double* m, int64_t n, int rescale, double mag_min, double mag_range, double span,
                          double min_val, int16_t* out, void* stream);
+/* The 2-D filters of every slice along `axis` (0, 1 or 2) of a [nz][ny][nx] volume in one launch sequence, as
+ * Slice.__apply_image_filter's "2D" branch (slice_.py:2363-2422) applies filters.py to each slice:
+ * b2v_median_filter_slices_i16: median_filter of each slice with a size x size window (window 1 along
+ *   `axis`, otherwise as b2v_median_filter_i16). in != out.
+ * b2v_uniform_filter_slices_i16: uniform_filter of each slice: two int16 passes along the in-slice axes in
+ *   ascending order, in -> tmp -> out. Three distinct volumes.
+ * b2v_sobel_magnitude with sz == NULL: the two-term magnitude sqrt(sx**2 + sy**2) of a 2-D sobel.
+ * b2v_slice_minmax: [min, max] of every slice as float64 pairs, minmax_out[2 s], minmax_out[2 s + 1] (device,
+ *   2 * n_slices doubles); dtype B2V_I16 or B2V_F64 (no NaN). One reduction over the volume, no host sync.
+ * b2v_sharpen_slices_i16, b2v_rescale_cast_slices_i16: b2v_sharpen_i16 / b2v_rescale_cast_i16 with each
+ *   slice's own constants read from b2v_slice_minmax pairs on the device: the slice's image [min, max] as
+ *   clip bounds; mag_min and mag_range = max - mag_min of the slice's magnitude, span and min_val from the
+ *   slice's image pair, and a plain cast where the slice's mag_range is not > 0 (filters.py:60-66).
+ * b2v_histogram_i16: np.histogram(a, bins, (lo, lo + bins))[0] for int16 a, 1 <= bins <= 65535: counts[k] =
+ *   #(a == lo + k), the last bin also counting lo + bins, values outside [lo, lo + bins] not counted (the image
+ *   histogram of Slice.matrix, slice_.py:190-192, 2490-2493, has lo = min, bins = max - min). counts: bins
+ *   int64 on the device, overwritten. */
+int b2v_median_filter_slices_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int axis, int16_t* out,
+                                 void* stream);
+int b2v_uniform_filter_slices_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int axis, int16_t* out,
+                                  int16_t* tmp, void* stream);
+int b2v_slice_minmax(const void* in, int dtype, int64_t nz, int64_t ny, int64_t nx, int axis, double* minmax_out,
+                     void* stream);
+int b2v_sharpen_slices_i16(const int16_t* img, const double* blurred, int64_t nz, int64_t ny, int64_t nx, int axis,
+                           double value, const double* minmax_dev, int16_t* out, void* stream);
+int b2v_rescale_cast_slices_i16(const double* m, int64_t nz, int64_t ny, int64_t nx, int axis, const double* mag_minmax_dev,
+                                const double* img_minmax_dev, int16_t* out, void* stream);
+int b2v_histogram_i16(const int16_t* a, int64_t n, int lo, int bins, int64_t* counts, void* stream);
 
 /* ---- connected components (SURVEY 8f-3) ------------------------------------------------------
  * b2v_label: scipy.ndimage.label(input, structure, output=uint32) as InVesalius calls it

@@ -59,6 +59,12 @@ PROTOTYPES = {
     "b2v_sharpen_i16": (cint, [vp, vp, i64, dbl, dbl, dbl, vp, vp]),
     "b2v_sobel_magnitude": (cint, [vp, vp, vp, i64, vp]),
     "b2v_rescale_cast_i16": (cint, [vp, i64, cint, dbl, dbl, dbl, dbl, vp, vp]),
+    "b2v_median_filter_slices_i16": (cint, [vp, i64, i64, i64, cint, cint, vp, vp]),
+    "b2v_uniform_filter_slices_i16": (cint, [vp, i64, i64, i64, cint, cint, vp, vp, vp]),
+    "b2v_slice_minmax": (cint, [vp, cint, i64, i64, i64, cint, vp, vp]),
+    "b2v_sharpen_slices_i16": (cint, [vp, vp, i64, i64, i64, cint, dbl, vp, vp, vp]),
+    "b2v_rescale_cast_slices_i16": (cint, [vp, i64, i64, i64, cint, vp, vp, vp, vp]),
+    "b2v_histogram_i16": (cint, [vp, i64, cint, cint, vp, vp]),
     "b2v_label_workspace_bytes": (i64, [i64]),
     "b2v_label": (cint, [vp, i64, i64, i64, vp, i64, i64, i64, vp, vp, vp, C.POINTER(i64)]),
     "b2v_count_regions": (cint, [vp, cint, i64, u32, vp, vp, vp]),

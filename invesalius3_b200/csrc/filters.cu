@@ -5,6 +5,9 @@
 //   b2v_median_filter_i16   ndimage.median_filter(matrix, size)   filters.py:9-12 (size 3, 4 or 5, mode 'reflect')
 //   b2v_uniform_filter_i16  ndimage.uniform_filter(matrix, size)  filters.py:15-18 (separable; every pass stores
 //                           trunc(sum / size) in int16 like SciPy's NI_UniformFilter1D writing into an int16 output)
+//   *_slices_i16, b2v_slice_minmax  the "2D" branch of slice_.py:2363-2422: every slice along one axis filtered in
+//                           the same launches, no pass along the slice axis, per-slice statistics on the device
+//   b2v_histogram_i16       np.histogram(matrix, max - min, (min, max))   slice_.py:190-192, 2490-2493
 // All integer results are bit-exact against SciPy / NumPy; convolve_non_zero sums in the reference's
 // loop order (k, j, i) in float64 without FMA.
 #include "b2v_common.cuh"
@@ -77,13 +80,15 @@ __global__ void __launch_bounds__(256) k_convolve_non_zero(const double* __restr
   }
 }
 
-// median of the S^3 neighbourhood (reflect borders; window [i - S/2, i - S/2 + S) and rank S^3 / 2 as
-// scipy.ndimage.median_filter takes them, even sizes included): radix select on the order-preserving
-// unsigned image of the int16 values, 16 counting passes over the window kept in registers / local memory
-template <int S>
+// median of the WZ x WY x WX neighbourhood (reflect borders; window [i - W/2, i - W/2 + W) per axis and
+// rank N / 2 as scipy.ndimage.median_filter takes them, even sizes included): radix select on the
+// order-preserving unsigned image of the int16 values, 16 counting passes over the window kept in
+// registers / local memory. <S, S, S> is the 3-D filter; a window of 1 along one axis is the 2-D filter of
+// every slice along that axis (median_filter(vol, size=(1, S, S)) == the per-slice loop, for axis 0).
+template <int WZ, int WY, int WX>
 __global__ void __launch_bounds__(128) k_median_i16(const int16_t* __restrict__ in, int nz, int ny, int nx,
                                                     int16_t* __restrict__ out) {
-  constexpr int N = S * S * S, R = N / 2, H = S / 2;
+  constexpr int N = WZ * WY * WX, R = N / 2;
   const long long n = (long long)nz * ny * nx;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += stride) {
@@ -93,14 +98,14 @@ __global__ void __launch_bounds__(128) k_median_i16(const int16_t* __restrict__ 
     unsigned short w[N];
     int c = 0;
 #pragma unroll
-    for (int kz = 0; kz < S; ++kz) {
-      const long long zz = reflect_idx(z - H + kz, nz);
+    for (int kz = 0; kz < WZ; ++kz) {
+      const long long zz = reflect_idx(z - WZ / 2 + kz, nz);
 #pragma unroll
-      for (int ky = 0; ky < S; ++ky) {
-        const long long yy = reflect_idx(y - H + ky, ny);
+      for (int ky = 0; ky < WY; ++ky) {
+        const long long yy = reflect_idx(y - WY / 2 + ky, ny);
         const int16_t* row = in + (zz * ny + yy) * nx;
 #pragma unroll
-        for (int kx = 0; kx < S; ++kx) w[c++] = (unsigned short)((int)row[reflect_idx(x - H + kx, nx)] + 32768);
+        for (int kx = 0; kx < WX; ++kx) w[c++] = (unsigned short)((int)row[reflect_idx(x - WX / 2 + kx, nx)] + 32768);
       }
     }
     // the largest value v such that at least N - R window entries are >= v  ==  the entry of rank R (0-based, ascending)
@@ -164,34 +169,198 @@ __global__ void __launch_bounds__(256) k_correlate1d(const TI* __restrict__ in, 
   }
 }
 
+// Where the elementwise kernels below take their per-voxel constants: one set for the whole volume, or
+// one set per slice along an axis, read from [min, max] pairs of b2v_slice_minmax on the device.
+struct SliceOf {       // slice index of flat voxel p: (p / div) % n
+  long long div;
+  int n;
+  __device__ __forceinline__ int operator()(long long p) const { return (int)((p / div) % n); }
+};
+
+SliceOf slice_of(int64_t ny, int64_t nx, int axis, int64_t nz) {
+  if (axis == 0) return {ny * nx, (int)nz};
+  if (axis == 1) return {nx, (int)ny};
+  return {1, (int)nx};
+}
+
+struct ClipWhole {
+  double lo, hi;
+  __device__ __forceinline__ void operator()(long long, double& l, double& h) const { l = lo; h = hi; }
+};
+
+struct ClipPerSlice {  // the slice's own [min, max]
+  const double* __restrict__ mm;
+  SliceOf sl;
+  __device__ __forceinline__ void operator()(long long p, double& l, double& h) const {
+    const int s = sl(p);
+    l = mm[2 * s];
+    h = mm[2 * s + 1];
+  }
+};
+
 // sharpening_filter (filters.py:21-29): clip(f + (value * 0.5) * (f - blurred), min, max).astype(int16)
+template <typename Clip>
 __global__ void __launch_bounds__(256) k_sharpen(const int16_t* __restrict__ img, const double* __restrict__ blurred, long long n,
-                                                 double half_value, double lo, double hi, int16_t* __restrict__ out) {
+                                                 double half_value, Clip clip, int16_t* __restrict__ out) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const double f = (double)img[i];
+    double lo, hi;
+    clip(i, lo, hi);
     double s = f + half_value * (f - blurred[i]);
     s = s < lo ? lo : (s > hi ? hi : s);
     out[i] = cast_out<int16_t>(s);
   }
 }
 
-// border_detection_filter (filters.py:45-51): sqrt(sx**2 + sy**2 + sz**2), in place into a
+// border_detection_filter (filters.py:45-55): sqrt(sx**2 + sy**2 + sz**2) on a volume, sqrt(sx**2 + sy**2)
+// on a slice (c == nullptr), in place into a
 __global__ void __launch_bounds__(256) k_sobel_magnitude(double* a, const double* __restrict__ b, const double* __restrict__ c,
                                                          long long n) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    a[i] = sqrt((a[i] * a[i] + b[i] * b[i]) + c[i] * c[i]);
+    a[i] = c ? sqrt((a[i] * a[i] + b[i] * b[i]) + c[i] * c[i]) : sqrt(a[i] * a[i] + b[i] * b[i]);
 }
 
-// (magnitude - mag_min) / mag_range * span + min_val, cast to int16 (filters.py:56-66); scale = 0: plain cast
-__global__ void __launch_bounds__(256) k_rescale_cast(const double* __restrict__ m, long long n, int rescale, double mag_min,
-                                                      double mag_range, double span, double min_val, int16_t* __restrict__ out) {
+struct Rescale {
+  int on;
+  double mag_min, mag_range, span, min_val;
+};
+
+struct RescaleWhole {
+  Rescale r;
+  __device__ __forceinline__ Rescale operator()(long long) const { return r; }
+};
+
+struct RescalePerSlice {  // filters.py:60-66 on the slice: its own magnitude range and image range
+  const double* __restrict__ mag_mm;
+  const double* __restrict__ img_mm;
+  SliceOf sl;
+  __device__ __forceinline__ Rescale operator()(long long p) const {
+    const int s = sl(p);
+    const double mag_min = mag_mm[2 * s], mag_range = mag_mm[2 * s + 1] - mag_min;
+    const double min_val = img_mm[2 * s], max_val = img_mm[2 * s + 1];
+    return {mag_range > 0, mag_min, mag_range, max_val - min_val, min_val};
+  }
+};
+
+// (magnitude - mag_min) / mag_range * span + min_val, cast to int16 (filters.py:56-66); on = 0: plain cast
+template <typename Scale>
+__global__ void __launch_bounds__(256) k_rescale_cast(const double* __restrict__ m, long long n, Scale scale,
+                                                      int16_t* __restrict__ out) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     double v = m[i];
-    if (rescale) v = (v - mag_min) / mag_range * span + min_val;
+    const Rescale c = scale(i);
+    if (c.on) v = (v - c.mag_min) / c.mag_range * c.span + c.min_val;
     out[i] = cast_out<int16_t>(v);
+  }
+}
+
+// ---- per-slice [min, max]: order-preserving uint64 keys reduced with atomicMin; the max is kept as the
+// min of the complemented key, so one 0xFF fill initialises both slots
+__device__ __forceinline__ unsigned long long order_key(double v) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double from_order_key(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+__device__ __forceinline__ void block_minmax_to(double lo, double hi, unsigned long long* slot) {
+  __shared__ double s_lo[32], s_hi[32];
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  const int tid = threadIdx.x + threadIdx.y * blockDim.x, nw = (blockDim.x * blockDim.y) >> 5;
+  if ((tid & 31) == 0) { s_lo[tid >> 5] = lo; s_hi[tid >> 5] = hi; }
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < nw; ++w) { lo = fmin(lo, s_lo[w]); hi = fmax(hi, s_hi[w]); }
+    atomicMin(slot, order_key(lo));
+    atomicMin(slot + 1, ~order_key(hi));
+  }
+}
+
+// slices along axis 0 or 1: block (slice s, part); slice element j is (y, x) for axis 0, (z, x) for axis 1
+template <typename T>
+__global__ void __launch_bounds__(256) k_slice_minmax_rows(const T* __restrict__ in, int nz, int ny, int nx, int axis,
+                                                           unsigned long long* __restrict__ keys) {
+  const int s = blockIdx.x;
+  const long long plane = (long long)ny * nx;
+  const long long m = axis == 0 ? plane : (long long)nz * nx;
+  double lo = INFINITY, hi = -INFINITY;
+  for (long long j = (long long)blockIdx.y * blockDim.x + threadIdx.x; j < m; j += (long long)gridDim.y * blockDim.x) {
+    const long long p = axis == 0 ? s * plane + j : (j / nx) * plane + (long long)s * nx + j % nx;
+    const double v = (double)in[p];
+    lo = fmin(lo, v);
+    hi = fmax(hi, v);
+  }
+  block_minmax_to(lo, hi, keys + 2 * s);
+}
+
+// slices along axis 2: block of 32 columns x 8 row lanes, each thread keeps one column's extremes over its rows
+template <typename T>
+__global__ void __launch_bounds__(256) k_slice_minmax_cols(const T* __restrict__ in, long long rows, int nx,
+                                                           unsigned long long* __restrict__ keys) {
+  __shared__ double s_lo[8][32], s_hi[8][32];
+  const int x = blockIdx.x * 32 + threadIdx.x;
+  double lo = INFINITY, hi = -INFINITY;
+  if (x < nx)
+    for (long long r = (long long)blockIdx.y * 8 + threadIdx.y; r < rows; r += (long long)gridDim.y * 8) {
+      const double v = (double)in[r * nx + x];
+      lo = fmin(lo, v);
+      hi = fmax(hi, v);
+    }
+  s_lo[threadIdx.y][threadIdx.x] = lo;
+  s_hi[threadIdx.y][threadIdx.x] = hi;
+  __syncthreads();
+  if (threadIdx.y == 0 && x < nx) {
+    for (int k = 1; k < 8; ++k) { lo = fmin(lo, s_lo[k][threadIdx.x]); hi = fmax(hi, s_hi[k][threadIdx.x]); }
+    atomicMin(keys + 2 * x, order_key(lo));
+    atomicMin(keys + 2 * x + 1, ~order_key(hi));
+  }
+}
+
+__global__ void k_slice_minmax_finish(unsigned long long* kv, int ns) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * ns; i += gridDim.x * blockDim.x) {
+    const unsigned long long k = kv[i];
+    reinterpret_cast<double*>(kv)[i] = from_order_key(i & 1 ? ~k : k);
+  }
+}
+
+// np.histogram(a, bins, (lo, lo + bins)) of int16 a: count k = #(a == lo + k), the last bin also takes lo + bins,
+// values outside [lo, lo + bins] are not counted. SHARED: per-block uint32 counts in dynamic shared memory,
+// added to the int64 counts at the end (the caller keeps each block under 2^32 values)
+template <bool SHARED>
+__global__ void __launch_bounds__(1024) k_histogram_i16(const int16_t* __restrict__ a, long long n, int lo, int bins,
+                                                        unsigned long long* __restrict__ counts) {
+  extern __shared__ unsigned int h[];
+  if (SHARED) {
+    for (int k = threadIdx.x; k < bins; k += blockDim.x) h[k] = 0;
+    __syncthreads();
+  }
+  auto add = [&](int v) {
+    const int k = v - lo;
+    if (k >= 0 && k <= bins) {
+      const int b = k == bins ? bins - 1 : k;
+      if (SHARED) atomicAdd(&h[b], 1u);
+      else atomicAdd(&counts[b], 1ull);
+    }
+  };
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long n4 = (reinterpret_cast<uintptr_t>(a) & 7) ? 0 : n / 4;   // four values per 8-byte load
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const short4 q = reinterpret_cast<const short4*>(a)[i];
+    add(q.x); add(q.y); add(q.z); add(q.w);
+  }
+  for (long long i = 4 * n4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) add(a[i]);
+  if (SHARED) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < bins; k += blockDim.x)
+      if (h[k]) atomicAdd(&counts[k], (unsigned long long)h[k]);
   }
 }
 
@@ -214,16 +383,42 @@ extern "C" int b2v_convolve_non_zero(const double* volume, int64_t sz, int64_t s
   return b2v_check_launch("k_convolve_non_zero");
 }
 
-extern "C" int b2v_median_filter_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int16_t* out,
-                                     void* stream) {
+namespace {
+
+// axis -1: the S^3 window; axis 0, 1, 2: the S x S window of every slice along that axis
+template <int S>
+void launch_median(const int16_t* in, int nz, int ny, int nx, int axis, int16_t* out, cudaStream_t s) {
+  const int g = fgrid((long long)nz * ny * nx, 128);
+  if (axis < 0) k_median_i16<S, S, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
+  else if (axis == 0) k_median_i16<1, S, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
+  else if (axis == 1) k_median_i16<S, 1, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
+  else k_median_i16<S, S, 1><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
+}
+
+int median_filter(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int axis, int16_t* out, void* stream) {
   B2V_REQUIRE(in && out && in != out && nz > 0 && ny > 0 && nx > 0 && nz * ny * nx < (1ll << 40), B2V_ERR_ARG,
               "median_filter: bad arguments");
   B2V_REQUIRE(size >= 3 && size <= 5, B2V_ERR_ARG, "median_filter: size must be 3, 4 or 5 (filters.py:11 keeps it there)");
   cudaStream_t s = (cudaStream_t)stream;
-  if (size == 3) k_median_i16<3><<<fgrid(nz * ny * nx, 128), 128, 0, s>>>(in, (int)nz, (int)ny, (int)nx, out);
-  else if (size == 4) k_median_i16<4><<<fgrid(nz * ny * nx, 128), 128, 0, s>>>(in, (int)nz, (int)ny, (int)nx, out);
-  else k_median_i16<5><<<fgrid(nz * ny * nx, 128), 128, 0, s>>>(in, (int)nz, (int)ny, (int)nx, out);
+  if (size == 3) launch_median<3>(in, (int)nz, (int)ny, (int)nx, axis, out, s);
+  else if (size == 4) launch_median<4>(in, (int)nz, (int)ny, (int)nx, axis, out, s);
+  else launch_median<5>(in, (int)nz, (int)ny, (int)nx, axis, out, s);
   return b2v_check_launch("k_median_i16");
+}
+
+bool valid_slice_axis(int axis) { return axis >= 0 && axis <= 2; }
+
+}  // namespace
+
+extern "C" int b2v_median_filter_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int16_t* out,
+                                     void* stream) {
+  return median_filter(in, nz, ny, nx, size, -1, out, stream);
+}
+
+extern "C" int b2v_median_filter_slices_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int axis,
+                                            int16_t* out, void* stream) {
+  B2V_REQUIRE(valid_slice_axis(axis), B2V_ERR_ARG, "median_filter_slices: axis must be 0, 1 or 2");
+  return median_filter(in, nz, ny, nx, size, axis, out, stream);
 }
 
 extern "C" int b2v_uniform_filter_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int16_t* out,
@@ -240,6 +435,73 @@ extern "C" int b2v_uniform_filter_i16(const int16_t* in, int64_t nz, int64_t ny,
   if ((rc = b2v_check_launch("k_uniform1d_i16"))) return rc;
   k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, 2, size, out);
   return b2v_check_launch("k_uniform1d_i16");
+}
+
+extern "C" int b2v_uniform_filter_slices_i16(const int16_t* in, int64_t nz, int64_t ny, int64_t nx, int size, int axis,
+                                             int16_t* out, int16_t* tmp, void* stream) {
+  B2V_REQUIRE(in && out && tmp && in != out && in != tmp && out != tmp && nz > 0 && ny > 0 && nx > 0 && size >= 1 &&
+                  valid_slice_axis(axis),
+              B2V_ERR_ARG, "uniform_filter_slices: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long n = nz * ny * nx;
+  const int a0 = axis == 0 ? 1 : 0, a1 = axis == 2 ? 1 : 2;   // the in-slice axes, ascending, as SciPy runs them
+  int rc;
+  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(in, (int)nz, (int)ny, (int)nx, a0, size, tmp);
+  if ((rc = b2v_check_launch("k_uniform1d_i16"))) return rc;
+  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, a1, size, out);
+  return b2v_check_launch("k_uniform1d_i16");
+}
+
+extern "C" int b2v_slice_minmax(const void* in, int dtype, int64_t nz, int64_t ny, int64_t nx, int axis, double* minmax_out,
+                                void* stream) {
+  B2V_REQUIRE(in && minmax_out && nz > 0 && ny > 0 && nx > 0 && valid_slice_axis(axis) && (dtype == B2V_I16 || dtype == B2V_F64),
+              B2V_ERR_ARG, "slice_minmax: bad arguments");
+  B2V_REQUIRE(nz < (1ll << 30) && ny < (1ll << 30) && nx < (1ll << 30), B2V_ERR_ARG, "slice_minmax: shape too large");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int ns = (int)(axis == 0 ? nz : (axis == 1 ? ny : nx));
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(minmax_out);
+  B2V_CUDA(cudaMemsetAsync(keys, 0xff, sizeof(double) * 2 * ns, s));
+  const long long target = (long long)b2v_sm_count() * 16;      // blocks in flight over the whole launch
+  if (axis == 2) {
+    const long long rows = nz * ny;
+    const int gx = (int)ceil_div64(nx, 32);
+    const int gy = (int)std::max<long long>(1, std::min<long long>(ceil_div64(rows, 64), ceil_div64(target, gx)));
+    const dim3 grid(gx, gy), block(32, 8);
+    if (dtype == B2V_I16) k_slice_minmax_cols<<<grid, block, 0, s>>>((const int16_t*)in, rows, (int)nx, keys);
+    else k_slice_minmax_cols<<<grid, block, 0, s>>>((const double*)in, rows, (int)nx, keys);
+  } else {
+    const long long m = axis == 0 ? ny * nx : nz * nx;          // voxels per slice
+    const int gy = (int)std::max<long long>(1, std::min<long long>(ceil_div64(m, 256 * 8), ceil_div64(target, ns)));
+    const dim3 grid(ns, gy);
+    if (dtype == B2V_I16) k_slice_minmax_rows<<<grid, 256, 0, s>>>((const int16_t*)in, (int)nz, (int)ny, (int)nx, axis, keys);
+    else k_slice_minmax_rows<<<grid, 256, 0, s>>>((const double*)in, (int)nz, (int)ny, (int)nx, axis, keys);
+  }
+  int rc;
+  if ((rc = b2v_check_launch("k_slice_minmax"))) return rc;
+  k_slice_minmax_finish<<<(int)ceil_div64(2 * ns, 256), 256, 0, s>>>(keys, ns);
+  return b2v_check_launch("k_slice_minmax_finish");
+}
+
+extern "C" int b2v_histogram_i16(const int16_t* a, int64_t n, int lo, int bins, int64_t* counts, void* stream) {
+  B2V_REQUIRE(a && counts && n > 0 && bins >= 1 && bins <= 65535, B2V_ERR_ARG, "histogram: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned long long* c = reinterpret_cast<unsigned long long*>(counts);
+  B2V_CUDA(cudaMemsetAsync(c, 0, sizeof(int64_t) * bins, s));
+  int dev = 0, optin = 0;
+  B2V_CUDA(cudaGetDevice(&dev));
+  B2V_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t smem = sizeof(unsigned int) * (size_t)bins;
+  if (smem <= (size_t)optin) {
+    B2V_CUDA(cudaFuncSetAttribute(k_histogram_i16<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_histogram_i16<true>, 1024, smem));
+    // one resident wave, and at least enough blocks that none counts 2^31 values into its uint32 bins
+    const long long g = std::max<long long>((long long)b2v_sm_count() * std::max(per_sm, 1), ceil_div64(n, 1ll << 31));
+    k_histogram_i16<true><<<(int)g, 1024, smem, s>>>(a, n, lo, bins, c);
+  } else {
+    k_histogram_i16<false><<<fgrid(n, 1024), 1024, 0, s>>>(a, n, lo, bins, c);
+  }
+  return b2v_check_launch("k_histogram_i16");
 }
 
 // dtype pairs (B2V_I16, B2V_I16), (B2V_I16, B2V_F64), (B2V_F64, B2V_F64), (B2V_F32, B2V_F32); in != out
@@ -266,12 +528,22 @@ extern "C" int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t
 extern "C" int b2v_sharpen_i16(const int16_t* img, const double* blurred, int64_t n, double value, double lo, double hi,
                                int16_t* out, void* stream) {
   B2V_REQUIRE(img && blurred && out && n > 0, B2V_ERR_ARG, "sharpen: bad arguments");
-  k_sharpen<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5, lo, hi, out);
+  k_sharpen<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5, ClipWhole{lo, hi}, out);
+  return b2v_check_launch("k_sharpen");
+}
+
+extern "C" int b2v_sharpen_slices_i16(const int16_t* img, const double* blurred, int64_t nz, int64_t ny, int64_t nx, int axis,
+                                      double value, const double* minmax_dev, int16_t* out, void* stream) {
+  B2V_REQUIRE(img && blurred && minmax_dev && out && nz > 0 && ny > 0 && nx > 0 && valid_slice_axis(axis), B2V_ERR_ARG,
+              "sharpen_slices: bad arguments");
+  const long long n = nz * ny * nx;
+  k_sharpen<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5,
+                                                        ClipPerSlice{minmax_dev, slice_of(ny, nx, axis, nz)}, out);
   return b2v_check_launch("k_sharpen");
 }
 
 extern "C" int b2v_sobel_magnitude(double* sx_inout, const double* sy, const double* sz, int64_t n, void* stream) {
-  B2V_REQUIRE(sx_inout && sy && sz && n > 0, B2V_ERR_ARG, "sobel_magnitude: bad arguments");
+  B2V_REQUIRE(sx_inout && sy && n > 0, B2V_ERR_ARG, "sobel_magnitude: bad arguments");
   k_sobel_magnitude<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(sx_inout, sy, sz, n);
   return b2v_check_launch("k_sobel_magnitude");
 }
@@ -279,6 +551,18 @@ extern "C" int b2v_sobel_magnitude(double* sx_inout, const double* sy, const dou
 extern "C" int b2v_rescale_cast_i16(const double* m, int64_t n, int rescale, double mag_min, double mag_range, double span,
                                     double min_val, int16_t* out, void* stream) {
   B2V_REQUIRE(m && out && n > 0, B2V_ERR_ARG, "rescale_cast: bad arguments");
-  k_rescale_cast<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(m, n, rescale, mag_min, mag_range, span, min_val, out);
+  k_rescale_cast<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(m, n, RescaleWhole{{rescale, mag_min, mag_range, span, min_val}},
+                                                             out);
+  return b2v_check_launch("k_rescale_cast");
+}
+
+extern "C" int b2v_rescale_cast_slices_i16(const double* m, int64_t nz, int64_t ny, int64_t nx, int axis,
+                                           const double* mag_minmax_dev, const double* img_minmax_dev, int16_t* out,
+                                           void* stream) {
+  B2V_REQUIRE(m && mag_minmax_dev && img_minmax_dev && out && nz > 0 && ny > 0 && nx > 0 && valid_slice_axis(axis),
+              B2V_ERR_ARG, "rescale_cast_slices: bad arguments");
+  const long long n = nz * ny * nx;
+  k_rescale_cast<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(
+      m, n, RescalePerSlice{mag_minmax_dev, img_minmax_dev, slice_of(ny, nx, axis, nz)}, out);
   return b2v_check_launch("k_rescale_cast");
 }
