@@ -274,7 +274,9 @@ int b2v_count_regions(const void* image, int dtype, int64_t n, uint32_t number_r
  * [0, d - 1) on any axis: cval. float64 arithmetic in the reference's order. spacing_host =
  * (sx, sy, sz), m_host = 16 doubles row-major, both on the HOST. volume / out: dense device
  * arrays of the same dtype (int16, uint8, float64). workspace: >= 256 bytes. SYNCHRONISES (a value
- * that does not fit the output type is B2V_ERR_RANGE: the reference panics). */
+ * that does not fit the output type is B2V_ERR_RANGE: the reference panics; so is a Lanczos-4 sample
+ * in range on an axis of 2 voxels, whose tap floor(f) - 3 stays outside after the one-step wrap,
+ * where the reference's index panics: nothing is read outside the volume). */
 int b2v_apply_view_matrix_transform(const void* volume, int dtype, int64_t dz, int64_t dy, int64_t dx,
                                     const double* spacing_host, const double* m_host, int64_t n, int orientation,
                                     int minterpol, double cval, void* out, int64_t odz, int64_t ody, int64_t odx,

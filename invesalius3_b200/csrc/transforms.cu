@@ -7,6 +7,12 @@
 // One thread per output voxel; gather-bound (8 / 64 / 343 reads per voxel through L1 / L2).
 // Bit-exact against the CPU restatement for modes 0-2; mode 3 goes through sin(): libm and the
 // device differ by an ulp on rare inputs, which may move a truncated value by one unit.
+// Reads stay inside [0, d) on every axis: a sample is interpolated only when 0 <= f < d - 1 on all
+// three axes (so d >= 2). Nearest and trilinear read floor(f) and floor(f) + 1 <= d - 1; tricubic's
+// taps floor(f) - 1 .. floor(f) + 2 lie in [-1, d] and the one-step wrap brings them into [0, d).
+// Lanczos-4's taps floor(f) - 3 .. floor(f) + 3 do too when d >= 3, but on a 2-voxel axis the tap
+// -3 is still -1 after the wrap: the reference's ndarray index panics there, and so does this
+// kernel (status word, nothing read, B2V_ERR_RANGE).
 #include <math.h>
 
 #include "b2v_common.cuh"
@@ -15,6 +21,14 @@ namespace {
 
 struct Mat4 { double m[16]; };
 struct VDims { long long dz, dy, dx; };
+
+// bits of the status word
+enum { kStatusCast = 1, kStatusIndex = 2 };
+
+// true when every tap lo .. hi (lo <= hi) lands in [0, n) after get_value's one-step wrap
+__device__ __forceinline__ bool taps_wrap_inside(long long lo, long long hi, long long n) {
+  return (lo >= 0 || lo + n >= 0) && (hi < n || hi - n < n);
+}
 
 template <typename T> __device__ __forceinline__ bool cast_f64(double v, T* o);
 template <> __device__ __forceinline__ bool cast_f64<int16_t>(double v, int16_t* o) {
@@ -80,7 +94,7 @@ __global__ void __launch_bounds__(256) k_view_transform(const T* __restrict__ vo
         const double c00 = v000 * (1.0 - xd) + v100 * xd, c10 = v010 * (1.0 - xd) + v110 * xd,
                      c01 = v001 * (1.0 - xd) + v101 * xd, c11 = v011 * (1.0 - xd) + v111 * xd;
         const double e0 = c00 * (1.0 - yd) + c10 * yd, e1 = c01 * (1.0 - yd) + c11 * yd;
-        if (!cast_f64<T>(e0 * (1.0 - zd) + e1 * zd, &val)) { *status = B2V_ERR_RANGE; val = 0; }
+        if (!cast_f64<T>(e0 * (1.0 - zd) + e1 * zd, &val)) { atomicOr(status, kStatusCast); val = 0; }
       } else if (minterpol == 2) {
         const long long xi = (long long)floor(fx), yi = (long long)floor(fy), zi = (long long)floor(fz);
         const double ty = fy - (double)yi, tz = fz - (double)zi;
@@ -95,12 +109,18 @@ __global__ void __launch_bounds__(256) k_view_transform(const T* __restrict__ vo
           }
           rr[a] = cubic(arr, ty);
         }
-        if (!cast_f64<T>(cubic(rr, fx - (double)xi), &val)) { *status = B2V_ERR_RANGE; val = 0; }
+        if (!cast_f64<T>(cubic(rr, fx - (double)xi), &val)) { atomicOr(status, kStatusCast); val = 0; }
         else if (val < cval) val = cval;
       } else {
         const int a = 4;
         const long long xd = (long long)floor(fx), yd = (long long)floor(fy), zd = (long long)floor(fz);
         const long long xi = xd - a + 1, yi = yd - a + 1, zi = zd - a + 1;
+        if (!taps_wrap_inside(xi, xd + a - 1, d.dx) || !taps_wrap_inside(yi, yd + a - 1, d.dy) ||
+            !taps_wrap_inside(zi, zd + a - 1, d.dz)) {
+          atomicOr(status, kStatusIndex);
+          out[i] = 0;
+          continue;
+        }
         double kx[7], ky[7], kz[7];
 #pragma unroll
         for (int k = 0; k < 7; ++k) {
@@ -119,7 +139,7 @@ __global__ void __launch_bounds__(256) k_view_transform(const T* __restrict__ vo
           }
           lz += ly * kz[kk];
         }
-        if (!cast_f64<T>(lz, &val)) { *status = B2V_ERR_RANGE; val = 0; }
+        if (!cast_f64<T>(lz, &val)) { atomicOr(status, kStatusCast); val = 0; }
         else if (val < cval) val = cval;
       }
     }
@@ -164,6 +184,9 @@ extern "C" int b2v_apply_view_matrix_transform(const void* volume, int dtype, in
   int st = 0;
   B2V_CUDA(cudaMemcpyAsync(&st, status, sizeof(int), cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));
+  B2V_REQUIRE(!(st & kStatusIndex), B2V_ERR_RANGE,
+              "apply_view_matrix_transform: a Lanczos-4 tap lies outside the volume after the one-step wrap "
+              "(an axis of 2 voxels): index out of bounds, the reference's ndarray indexing panics here");
   B2V_REQUIRE(st == 0, B2V_ERR_RANGE,
               "apply_view_matrix_transform: an interpolated value is not representable in the output type (the reference panics here)");
   return B2V_OK;

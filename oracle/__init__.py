@@ -278,6 +278,18 @@ def apply_view_matrix_transform(volume, spacing, m, n, orientation, minterpol, c
     """invesalius_rs/__init__.py:84 -> transforms_py.rs:96-148 -> transforms.rs:9-55 ->
     interpolation.rs (nearest 0, trilinear 1, tricubic 2, Lanczos-4 otherwise). PARITY UNPINNED
     (no reference test): restated in oracle/transforms.c."""
+    rc = apply_view_matrix_transform_rc(volume, spacing, m, n, orientation, minterpol, cval, out)
+    if rc == 4:
+        raise ValueError("Lanczos-4 tap outside the volume after the one-step wrap: index out of bounds "
+                         "(Rust panic in ndarray indexing, interpolation.rs:34)")
+    if rc:
+        raise ValueError("interpolated value not representable in the output type (Rust panic in interpolation.rs)")
+
+
+def apply_view_matrix_transform_rc(volume, spacing, m, n, orientation, minterpol, cval, out):
+    """apply_view_matrix_transform returning the checker's code instead of raising: 0, 3 (a cast
+    panics) or 4 (a Lanczos-4 tap outside the volume); `out` is written in every case, 0 where a
+    sample panics."""
     suf = _SUFFIX.get(volume.dtype)
     if suf is None or out.dtype != volume.dtype or volume.ndim != 3 or out.ndim != 3:
         raise TypeError("Invalid volume or output type")
@@ -287,8 +299,7 @@ def apply_view_matrix_transform(volume, spacing, m, n, orientation, minterpol, c
     fn = getattr(lib(), f"orc_avmt_{suf}")
     rc = fn(_ptr(volume), _estrides(volume), *map(C.c_int64, volume.shape), _ptr(sp), _ptr(mm), C.c_int64(int(n)),
             ORIENT.get(orientation, 3), int(minterpol), _CT[suf](cval), _ptr(out), _estrides(out), *map(C.c_int64, out.shape))
-    if rc:
-        raise ValueError("interpolated value not representable in the output type (Rust panic in interpolation.rs)")
+    return rc
 
 
 # --------------------------------------------------------------------------- marching cubes

@@ -7,7 +7,9 @@
  * nalgebra's Matrix4 * Vector4 accumulates column by column, i.e. every row as
  * ((m0 c0 + m1 c1) + m2 c2) + m3 c3.
  *
- * Returns 0, or 3 when a cast to the output type would have panicked (NumCast::from(..).unwrap()). */
+ * Returns 0, 3 when a cast to the output type would have panicked (NumCast::from(..).unwrap()), or 4
+ * when a Lanczos-4 tap is still outside the volume after get_value's one-step wrap (an axis of 2
+ * voxels: ndarray's index panics). Such a sample reads nothing and is written as 0. */
 #include <math.h>
 #include <stdint.h>
 
@@ -25,6 +27,8 @@ static double bicubic_interpolate(double p[4][4], double x, double y) {
   for (int i = 0; i < 4; ++i) arr[i] = cubic_interpolate(p[i], y);
   return cubic_interpolate(arr, x);
 }
+/* every tap lo .. hi lands in [0, n) after the one-step wrap */
+static int taps_wrap_inside(int64_t lo, int64_t hi, int64_t n) { return (lo >= 0 || lo + n >= 0) && (hi < n || hi - n < n); }
 static double lanczos_kernel(double x, int a) {
   if (x == 0.0) return 1.0;
   if (-(double)a <= x && x < (double)a) {
@@ -72,7 +76,7 @@ static double lanczos_kernel(double x, int a) {
               const double c00 = v000 * (1.0 - xd) + v100 * xd, c10 = v010 * (1.0 - xd) + v110 * xd,             \
                            c01 = v001 * (1.0 - xd) + v101 * xd, c11 = v011 * (1.0 - xd) + v111 * xd;             \
               const double c0 = c00 * (1.0 - yd) + c10 * yd, c1 = c01 * (1.0 - yd) + c11 * yd;                   \
-              if (!CAST(c0 * (1.0 - zd) + c1 * zd, &val)) { bad = 1; val = 0; }                                  \
+              if (!CAST(c0 * (1.0 - zd) + c1 * zd, &val)) { bad |= 1; val = 0; }                                  \
             } else if (minterpol == 2) {                                                                         \
               const int64_t xi = (int64_t)floor(fx), yi = (int64_t)floor(fy), zi = (int64_t)floor(fz);           \
               double p[4][4][4];                                                                                 \
@@ -80,12 +84,18 @@ static double lanczos_kernel(double x, int a) {
                 p[i][j][k] = NAME##_get(vol, vs, dz, dy, dx, xi + i - 1, yi + j - 1, zi + k - 1);                \
               double r[4];                                                                                       \
               for (int i = 0; i < 4; ++i) r[i] = bicubic_interpolate(p[i], fy - (double)yi, fz - (double)zi);    \
-              if (!CAST(cubic_interpolate(r, fx - (double)xi), &val)) { bad = 1; val = 0; }                      \
+              if (!CAST(cubic_interpolate(r, fx - (double)xi), &val)) { bad |= 1; val = 0; }                      \
               else if (val < cval) val = cval;                                                                   \
             } else {                                                                                             \
               const int a = 4;                                                                                   \
               const int64_t xd = (int64_t)floor(fx), yd = (int64_t)floor(fy), zd = (int64_t)floor(fz);           \
               const int64_t xi = xd - a + 1, xf = xd + a, yi = yd - a + 1, yf = yd + a, zi = zd - a + 1, zf = zd + a; \
+              if (!taps_wrap_inside(xi, xf - 1, dx) || !taps_wrap_inside(yi, yf - 1, dy) ||                      \
+                  !taps_wrap_inside(zi, zf - 1, dz)) {                                                           \
+                bad |= 2;                                                                                        \
+                out[IDX3(cz, cy, cx, os)] = 0;                                                                   \
+                continue;                                                                                        \
+              }                                                                                                  \
               double tx[7][7], ty[7];                                                                            \
               for (int64_t kk = zi; kk < zf; ++kk)                                                               \
                 for (int64_t jj = yi; jj < yf; ++jj) {                                                           \
@@ -101,13 +111,13 @@ static double lanczos_kernel(double x, int a) {
               }                                                                                                  \
               double lz = 0.0;                                                                                   \
               for (int64_t kk = zi; kk < zf; ++kk) lz += ty[kk - zi] * lanczos_kernel(fz - (double)kk, a);       \
-              if (!CAST(lz, &val)) { bad = 1; val = 0; }                                                         \
+              if (!CAST(lz, &val)) { bad |= 1; val = 0; }                                                         \
               else if (val < cval) val = cval;                                                                   \
             }                                                                                                    \
           }                                                                                                      \
           out[IDX3(cz, cy, cx, os)] = val;                                                                       \
         }                                                                                                        \
-    return bad ? 3 : 0;                                                                                          \
+    return (bad & 2) ? 4 : bad ? 3 : 0;                                                                          \
   }
 DEF_AVMT(orc_avmt_i16, int16_t, cast_i16)
 DEF_AVMT(orc_avmt_u8, uint8_t, cast_u8)
