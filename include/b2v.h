@@ -436,6 +436,41 @@ int64_t b2v_binary_morphology_workspace_bytes(int64_t dz, int64_t dy, int64_t dx
 int b2v_binary_morphology(const uint8_t* in, int64_t dz, int64_t dy, int64_t dx, uint8_t threshold, int op, int radius,
                           int planar, uint8_t set_value, uint8_t* out, int64_t* counts, void* workspace, void* stream);
 
+/* ---- remove non-visible faces --------------------------------------------------------------------
+ * plugins/remove_non_visible_faces/remove_non_visible_faces.py:19-119 on arrays, without OpenGL: the
+ * surface is depth-rendered at 800x800 from each camera, a vertex is visible when some view sees it
+ * (vtkSelectVisiblePoints, tolerance 0.01), a face is kept when any vertex is selected (the visible ones,
+ * or the invisible ones with remove_visible != 0), and the kept faces are cleaned as vtkCleanPolyData
+ * does (exactly coincident points merged, the first use wins; vertices numbered in order of first use
+ * over the kept faces' corners; faces degenerate after the merge dropped). VTK's camera and clipping
+ * constants are restated, not verified against VTK; all arithmetic is float64 without FMA.
+ *   verts: float32 [nv][3] (1 <= nv < 2^31, finite); faces: int32 (faces_i64 = 0) or int64 [nt][face_cols],
+ *   face_cols 3, or 4 with a leading 3 in every row; views: 1..64.
+ *   b2v_visibility_bounds   vertex bounds (xmin, xmax, ymin, ymax, zmin, zmax) to bounds_host, -0 read
+ *                           as +0; B2V_ERR_ARG on a non-finite vertex. Synchronises the stream.
+ *   b2v_visibility_cameras  host only: for each direction of positions_host [nviews][3] (zero: ERR_ARG),
+ *                           B2V_VIS_CAMERA_DOUBLES doubles: [0..15] the composite projection (row-major,
+ *                           depth in [0, 1]), [16..18] position, [19..21] focal point, [22..24] view-up,
+ *                           [25..26] clipping range, [27] camera distance, [28] bounding radius.
+ *   b2v_visibility_count    renders, selects and counts the output (V', T'); ERR_ARG on a bad face.
+ *                           Synchronises the stream. The workspace then holds what b2v_visibility_layout
+ *                           locates: [0] byte offset of the float64 depth buffers [views][800 (y)][800 (x)],
+ *                           [1] of the uint8 per-vertex visibility, [2] of the uint64 count of triangles
+ *                           drawn by the cooperative (large-triangle) path.
+ *   b2v_visibility_emit     writes verts_out float32 [V'][3] and faces_out int32 [T'][3]; same arguments
+ *                           and workspace as the count. */
+#define B2V_VIS_CAMERA_DOUBLES 32
+int64_t b2v_visibility_workspace_bytes(int64_t nv, int64_t nt, int nviews);
+int b2v_visibility_layout(int64_t nv, int64_t nt, int nviews, int64_t* layout_out);
+int b2v_visibility_bounds(const float* verts, int64_t nv, void* workspace, void* stream, double* bounds_host);
+int b2v_visibility_cameras(const double* bounds_host, const double* positions_host, int nviews, double* cameras_host);
+int b2v_visibility_count(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                         const double* cameras_host, int nviews, int remove_visible, void* workspace, void* stream,
+                         int64_t* nverts_host, int64_t* nfaces_host);
+int b2v_visibility_emit(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                        int nviews, int remove_visible, void* workspace, float* verts_out, int32_t* faces_out,
+                        void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

@@ -122,7 +122,16 @@ PROTOTYPES = {
     "b2v_image_normalize_f32_i16": (cint, [vp, i64, f32, f32, f32, f32, C.c_int16, vp, vp]),
     "b2v_binary_morphology_workspace_bytes": (i64, [i64, i64, i64, cint]),
     "b2v_binary_morphology": (cint, [vp, i64, i64, i64, u8, cint, cint, cint, u8, vp, vp, vp, vp]),
+    "b2v_visibility_workspace_bytes": (i64, [i64, i64, cint]),
+    "b2v_visibility_layout": (cint, [i64, i64, cint, C.POINTER(i64)]),
+    "b2v_visibility_bounds": (cint, [vp, i64, vp, vp, C.POINTER(dbl)]),
+    "b2v_visibility_cameras": (cint, [C.POINTER(dbl), C.POINTER(dbl), cint, C.POINTER(dbl)]),
+    "b2v_visibility_count": (cint, [vp, i64, vp, i64, cint, cint, C.POINTER(dbl), cint, cint, vp, vp, C.POINTER(i64),
+                                    C.POINTER(i64)]),
+    "b2v_visibility_emit": (cint, [vp, i64, vp, i64, cint, cint, cint, cint, vp, vp, vp, vp]),
 }
+
+VIS_CAMERA_DOUBLES = 32
 
 F32 = 3
 ZOOM_CONSTANT, ZOOM_MIRROR = 0, 1
