@@ -471,6 +471,36 @@ int b2v_visibility_emit(const float* verts, int64_t nv, const void* faces, int64
                         int nviews, int remove_visible, void* workspace, float* verts_out, int32_t* faces_out,
                         void* stream);
 
+/* ---- surface connectivity ------------------------------------------------------------------------
+ * vtkPolyDataConnectivityFilter on triangles, behind polydata_utils.SelectLargestPart, SplitDisconectedParts
+ * and JoinSeedsParts (invesalius/data/polydata_utils.py:206-278; surface.py:319-411). The contract (VTK's
+ * region numbering, wave order and PointMap, restated and unverified) is in DESIGN.md §3 and the header of
+ * the C checker, connectivity.c.
+ *   verts: float32 [nv][3]; faces: int32 (faces_i64 = 0) or int64 [nt][face_cols], face_cols 3, or 4 with a
+ *   leading 3 in every row; nv, nt < 2^31. seeded = 0: every region (all-regions mode; seeds ignored);
+ *   seeded = 1: one region grown from the point ids seeds_host[nseeds] (negative ids skipped, an id >= nv is
+ *   B2V_ERR_ARG). A bad face is B2V_ERR_ARG.
+ *   b2v_conn_count   runs the filter; counts_host[5] = {regions R, points numbered N, cells visited C,
+ *                    the deepest region's wave count, the largest region (ties: the lowest number; -1 if
+ *                    none)}. Synchronises the stream.
+ *   b2v_conn_emit    from the same workspace: verts_out float32 [N][3] in PointMap order and point_ids
+ *                    int32 [N] (their input ids); faces_out int32 [C][3] (corners through PointMap) and
+ *                    cell_ids int32 [C]: the visited cells grouped by region, ascending id inside each;
+ *                    point_offsets / cell_offsets int64 [R + 1]: region r owns the points
+ *                    [point_offsets[r], point_offsets[r + 1]) and the faces [cell_offsets[r], cell_offsets[r+1]).
+ *   b2v_conn_layout  byte offsets in the workspace, valid after the count: [0] int32 [nt] region of each cell
+ *                    (-1: not visited), [1] int32 [nv] PointMap (-1: not numbered), [2] int32 [C] the visited
+ *                    cells in wave order, [3] int32 [C] region-major, [4] int32 [3 nt] the point -> cell
+ *                    links, [5] uint64 [nv + 1] their offsets. */
+int64_t b2v_conn_workspace_bytes(int64_t nv, int64_t nt, int64_t nseeds);
+int b2v_conn_layout(int64_t nv, int64_t nt, int64_t nseeds, int64_t* layout_out);
+int b2v_conn_count(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                   int seeded, const int64_t* seeds_host, int64_t nseeds, void* workspace, void* stream,
+                   int64_t* counts_host);
+int b2v_conn_emit(const float* verts, int64_t nv, int64_t nt, int64_t nseeds, const int64_t* counts_host,
+                  void* workspace, float* verts_out, int32_t* point_ids, int32_t* faces_out, int32_t* cell_ids,
+                  int64_t* point_offsets, int64_t* cell_offsets, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

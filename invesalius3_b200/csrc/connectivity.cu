@@ -1,0 +1,857 @@
+// The surface connectivity tools on the device: vtkPolyDataConnectivityFilter on triangles, as InVesalius's
+// "Select largest surface", "Split all disconnected surfaces" and "Select regions of interest..." use it
+// (polydata_utils.py:206-278). The contract is restated once, in the C checker's header (connectivity.c,
+// DESIGN.md §3 "Surface connectivity"): regions in
+// the order of their lowest cell, cells marked in VTK's wave order, points numbered in order of first use.
+// Every step below reproduces that order exactly, with no per-wave host round trip.
+//
+//   k_conn_load          faces -> int32 [T][3] (a bad face sets a status bit), link counts per point.
+//   links                the corners (in corner order, i.e. ascending cell) stably sorted by point id: the
+//                        point -> cell links of vtkCellLinks, duplicates of degenerate triangles included.
+//   k_cc_*               union-find over the triangle-point incidence (hook, then compress); each
+//                        component's minimum cell; a scan of the "minimum cell" flags numbers the regions
+//                        and lists their first cells: wave 0 of every region at once.
+//   k_conn_levels        one persistent cooperative launch runs every wave of every region: the appended
+//                        list of wave L+1 is laid out by a scan over wave L (parent order, then j, then link
+//                        order), each unmarked candidate takes the atomicMin of its positions, and a second
+//                        scan compacts the winners in position order. That is VTK's processing order, in
+//                        linear work and without a sort. A wave of at most kSmall cells runs in block 0
+//                        alone, with block barriers, until the waves grow again.
+//   sort by region       the processed sequence (wave-major) stably sorted by region: region-major ranks.
+//   k_conn_first_use     each point takes the atomicMin of (rank, j) over its corners; a scan of the
+//                        first-use flags is PointMap, region by region.
+//   faces                the visited cells, in ascending id, stably sorted by region.
+//
+// Stable sorts are LSD radix passes of 8 bits (per-block digit histograms, one scan, a scatter ranked by
+// warp match), only over the bits the largest key needs.
+#include <cooperative_groups.h>
+#include <string.h>
+
+#include "b2v_common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace {
+
+constexpr int kBlock = 256;
+constexpr int kScanItems = 4;                      // items per thread of the device-wide scan
+constexpr int kScanTile = kBlock * kScanItems;
+constexpr int kMaxGrid = 1024;                     // blocks of the persistent launch (btot capacity)
+constexpr int64_t kSmall = 2048;                   // waves this small run in one block
+constexpr unsigned long long kInf = ~0ull;
+
+enum : uint32_t { ST_BAD_FACE = 1u };
+
+struct ConnWs {
+  long long* ctl;                  // [0..15]: two state records for the persistent launch, then results
+  uint32_t* status;
+  unsigned long long* totals;      // [8] scan totals
+  int32_t* tri;                    // [T][3]
+  unsigned long long* lstart;      // [V + 1] link offsets
+  int32_t* links;                  // [3T]
+  uint32_t *ka, *va, *kb, *vb;     // [3T] sort ping-pong
+  unsigned long long* hist;        // [256 * nb3 + 1]
+  unsigned long long* scratch;     // scan block sums
+  int32_t* parent;                 // [V]
+  uint32_t* cmin;                  // [V]
+  unsigned long long* tflag;       // [T + 1]
+  int32_t* reg;                    // [T]
+  unsigned long long* best;        // [T]
+  int32_t* seq;                    // [T] processed cells, wave-major
+  int64_t* seeds;                  // [nseeds]
+  unsigned long long *loc1, *loc2; // [max(T, nseeds)]
+  unsigned long long* btot;        // [2][kMaxGrid]
+  unsigned long long* celloff;     // [T + 2]
+  int32_t* rank;                   // [T] processed cells, region-major
+  unsigned long long* fu;          // [V] first-use corner
+  unsigned long long* cflag;       // [3T + 1]
+  int32_t* pmap;                   // [V]
+  int32_t* inv;                    // [V]
+  int32_t* cells;                  // [T] visited cells, grouped by region
+  unsigned long long* ptoff;       // [T + 2]
+  int64_t nb3;
+  size_t bytes;
+};
+
+inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
+
+int64_t scan_blocks(int64_t n) { return ceil_div64(n > 0 ? n : 1, kScanTile); }
+
+ConnWs carve(void* base, int64_t nv, int64_t nt, int64_t nseeds) {
+  ConnWs w;
+  char* p = (char*)base;
+  size_t o = 0;
+  auto take = [&](size_t n) { char* r = p + o; o += al(n); return r; };
+  const size_t V = (size_t)nv, T = (size_t)nt, C3 = 3 * T;
+  const size_t items = T > (size_t)nseeds ? T : (size_t)nseeds;
+  w.nb3 = ceil_div64((int64_t)(C3 > 0 ? C3 : 1), kBlock);
+  const int64_t hist_n = 256 * w.nb3 + 1;
+  int64_t longest = hist_n;
+  if ((int64_t)C3 + 1 > longest) longest = (int64_t)C3 + 1;
+  if ((int64_t)V + 1 > longest) longest = (int64_t)V + 1;
+  w.ctl = (long long*)take(16 * 8);
+  w.status = (uint32_t*)take(16);
+  w.totals = (unsigned long long*)take(8 * 8);
+  w.tri = (int32_t*)take(C3 * 4);
+  w.lstart = (unsigned long long*)take((V + 1) * 8);
+  w.links = (int32_t*)take(C3 * 4);
+  w.ka = (uint32_t*)take(C3 * 4);
+  w.va = (uint32_t*)take(C3 * 4);
+  w.kb = (uint32_t*)take(C3 * 4);
+  w.vb = (uint32_t*)take(C3 * 4);
+  w.hist = (unsigned long long*)take((size_t)hist_n * 8);
+  w.scratch = (unsigned long long*)take((size_t)(scan_blocks(longest) + 1) * 8);
+  w.parent = (int32_t*)take(V * 4);
+  w.cmin = (uint32_t*)take(V * 4);
+  w.tflag = (unsigned long long*)take((T + 1) * 8);
+  w.reg = (int32_t*)take(T * 4);
+  w.best = (unsigned long long*)take(T * 8);
+  w.seq = (int32_t*)take(T * 4);
+  w.seeds = (int64_t*)take((size_t)nseeds * 8);
+  w.loc1 = (unsigned long long*)take(items * 8);
+  w.loc2 = (unsigned long long*)take(items * 8);
+  w.btot = (unsigned long long*)take(2 * kMaxGrid * 8);
+  w.celloff = (unsigned long long*)take((T + 2) * 8);
+  w.rank = (int32_t*)take(T * 4);
+  w.fu = (unsigned long long*)take(V * 8);
+  w.cflag = (unsigned long long*)take((C3 + 1) * 8);
+  w.pmap = (int32_t*)take(V * 4);
+  w.inv = (int32_t*)take(V * 4);
+  w.cells = (int32_t*)take(T * 4);
+  w.ptoff = (unsigned long long*)take((T + 2) * 8);
+  w.bytes = o;
+  return w;
+}
+
+__device__ __forceinline__ int64_t gtid() { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; }
+__device__ __forceinline__ int64_t gstride() { return (int64_t)gridDim.x * blockDim.x; }
+
+unsigned grid_for(int64_t n, int per_sm = 16) {
+  int64_t b = ceil_div64(n, kBlock);
+  const int64_t cap = (int64_t)b2v_sm_count() * per_sm;
+  if (b > cap) b = cap;
+  return (unsigned)(b < 1 ? 1 : b);
+}
+
+// block-wide exclusive scan (kBlock threads); returns the prefix and the block total
+template <typename T>
+__device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  T inc = x;
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  if (lane == 31) s_w[wid] = inc;
+  __syncthreads();
+  if (wid == 0) {
+    const int nw = blockDim.x >> 5;
+    T v = lane < nw ? s_w[lane] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const T y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += y;
+    }
+    if (lane < nw) s_w[lane] = v;
+  }
+  __syncthreads();
+  const T base = wid ? s_w[wid - 1] : 0;
+  *total = s_w[(blockDim.x >> 5) - 1];
+  __syncthreads();
+  return base + inc - x;
+}
+
+// ---- device-wide exclusive scan of uint64 in place (tiles of kScanTile, then the tile sums) ----------------
+__global__ void __launch_bounds__(kBlock) k_scan_tiles(unsigned long long* a, int64_t n,
+                                                       unsigned long long* sums) {
+  __shared__ unsigned long long s_w[kBlock / 32];
+  const int64_t base = (int64_t)blockIdx.x * kScanTile + (int64_t)threadIdx.x * kScanItems;
+  unsigned long long v[kScanItems], s = 0;
+  for (int k = 0; k < kScanItems; ++k) {
+    v[k] = base + k < n ? a[base + k] : 0ull;
+    s += v[k];
+  }
+  unsigned long long tot;
+  unsigned long long ex = block_exscan<unsigned long long>(s, s_w, &tot);
+  for (int k = 0; k < kScanItems; ++k) {
+    if (base + k < n) a[base + k] = ex;
+    ex += v[k];
+  }
+  if (threadIdx.x == 0) sums[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(1024) k_scan_sums(unsigned long long* a, int64_t nb, unsigned long long* total) {
+  __shared__ unsigned long long s_w[32];
+  unsigned long long carry = 0;
+  for (int64_t base = 0; base < nb; base += blockDim.x) {
+    const int64_t i = base + threadIdx.x;
+    const unsigned long long x = i < nb ? a[i] : 0ull;
+    unsigned long long tot;
+    const unsigned long long ex = block_exscan<unsigned long long>(x, s_w, &tot);
+    if (i < nb) a[i] = carry + ex;
+    carry += tot;
+  }
+  if (threadIdx.x == 0 && total) *total = carry;
+}
+
+__global__ void __launch_bounds__(kBlock) k_scan_add(unsigned long long* a, int64_t n,
+                                                     const unsigned long long* __restrict__ sums) {
+  const unsigned long long add = sums[blockIdx.x];
+  const int64_t base = (int64_t)blockIdx.x * kScanTile;
+  for (int k = threadIdx.x; k < kScanTile; k += kBlock)
+    if (base + k < n) a[base + k] += add;
+}
+
+int scan(unsigned long long* a, int64_t n, unsigned long long* scratch, unsigned long long* total, cudaStream_t s) {
+  const int64_t nb = scan_blocks(n);
+  B2V_REQUIRE(nb <= 0x7fffffffLL, B2V_ERR_ARG, "connectivity: scan too long");
+  k_scan_tiles<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
+  if (int rc = b2v_check_launch("k_scan_tiles")) return rc;
+  k_scan_sums<<<1, 1024, 0, s>>>(scratch, nb, total);
+  if (int rc = b2v_check_launch("k_scan_sums")) return rc;
+  k_scan_add<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
+  return b2v_check_launch("k_scan_add");
+}
+
+// ---- stable LSD radix sort of (key, value) pairs, 8 bits a pass -------------------------------------------
+__global__ void __launch_bounds__(kBlock) k_rs_hist(const uint32_t* __restrict__ keys, int64_t n, int shift,
+                                                    int64_t nb, unsigned long long* hist) {
+  __shared__ uint32_t s_c[256];
+  s_c[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i < n) atomicAdd(&s_c[(keys[i] >> shift) & 255u], 1u);
+  __syncthreads();
+  hist[(int64_t)threadIdx.x * nb + blockIdx.x] = s_c[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(kBlock) k_rs_scatter(const uint32_t* __restrict__ kin,
+                                                       const uint32_t* __restrict__ vin, int64_t n, int shift,
+                                                       int64_t nb, const unsigned long long* __restrict__ hist,
+                                                       uint32_t* __restrict__ kout, uint32_t* __restrict__ vout) {
+  __shared__ uint32_t s_c[kBlock / 32][256];
+  for (int k = threadIdx.x; k < (kBlock / 32) * 256; k += kBlock) (&s_c[0][0])[k] = 0;
+  __syncthreads();
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t key = i < n ? kin[i] : 0u;
+  const uint32_t d = i < n ? (key >> shift) & 255u : 256u;   // 256: no item
+  const uint32_t peers = __match_any_sync(0xffffffffu, d);
+  const uint32_t below = peers & ((1u << lane) - 1u);
+  if (d < 256u && below == 0) s_c[wid][d] = __popc(peers);
+  __syncthreads();
+  if (d >= 256u) return;
+  uint32_t r = __popc(below);
+  for (int w = 0; w < wid; ++w) r += s_c[w][d];
+  const unsigned long long pos = hist[(int64_t)d * nb + blockIdx.x] + r;
+  kout[pos] = key;
+  vout[pos] = vin[i];
+}
+
+// sorts (ka, va)[0..n) stably by key < 2^keybits; the result is in (ka, va) or (kb, vb): *out_v says which
+int sort_pairs(ConnWs& w, int64_t n, int keybits, uint32_t** out_v, cudaStream_t s) {
+  uint32_t *ki = w.ka, *vi = w.va, *ko = w.kb, *vo = w.vb;
+  const int64_t nb = ceil_div64(n, kBlock);
+  for (int shift = 0; shift < keybits && n > 1; shift += 8) {
+    k_rs_hist<<<(unsigned)nb, kBlock, 0, s>>>(ki, n, shift, nb, w.hist);
+    if (int rc = b2v_check_launch("k_rs_hist")) return rc;
+    if (int rc = scan(w.hist, 256 * nb, w.scratch, nullptr, s)) return rc;
+    k_rs_scatter<<<(unsigned)nb, kBlock, 0, s>>>(ki, vi, n, shift, nb, w.hist, ko, vo);
+    if (int rc = b2v_check_launch("k_rs_scatter")) return rc;
+    uint32_t* t = ki; ki = ko; ko = t;
+    t = vi; vi = vo; vo = t;
+  }
+  *out_v = vi;
+  return B2V_OK;
+}
+
+int bits_for(int64_t max_key) {
+  int b = 0;
+  while (b < 32 && (max_key >> b) > 0) ++b;
+  return b;
+}
+
+// ---- faces and links -------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kBlock) k_conn_load(const void* faces, int64_t nt, int cols, int i64, int64_t nv,
+                                                     int32_t* __restrict__ tri, unsigned long long* deg,
+                                                     uint32_t* ka, uint32_t* va, uint32_t* status) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) {
+    const int off = cols == 4 ? 1 : 0;
+    int64_t v[3], lead;
+    if (i64) {
+      const int64_t* f = (const int64_t*)faces + t * cols;
+      lead = off ? f[0] : 3;
+      v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
+    } else {
+      const int32_t* f = (const int32_t*)faces + t * cols;
+      lead = off ? f[0] : 3;
+      v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
+    }
+    bool ok = lead == 3;
+    for (int j = 0; j < 3; ++j) ok = ok && v[j] >= 0 && v[j] < nv;
+    if (!ok) {
+      atomicOr(status, ST_BAD_FACE);
+      v[0] = v[1] = v[2] = 0;
+    }
+    for (int j = 0; j < 3; ++j) {
+      tri[3 * t + j] = (int32_t)v[j];
+      atomicAdd(&deg[v[j]], 1ull);
+      ka[3 * t + j] = (uint32_t)v[j];
+      va[3 * t + j] = (uint32_t)t;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_copy_i32(const uint32_t* __restrict__ in, int64_t n, int32_t* out) {
+  for (int64_t i = gtid(); i < n; i += gstride()) out[i] = (int32_t)in[i];
+}
+
+// ---- union-find partition --------------------------------------------------------------------------------
+__device__ __forceinline__ int32_t uf_find(const int32_t* parent, int32_t x) {
+  const volatile int32_t* p = parent;
+  int32_t y = p[x];
+  while (y != x) { x = y; y = p[x]; }
+  return x;
+}
+
+__device__ __forceinline__ void uf_unite(int32_t* parent, int32_t a, int32_t b) {
+  for (;;) {
+    a = uf_find(parent, a);
+    b = uf_find(parent, b);
+    if (a == b) return;
+    if (a > b) { const int32_t t = a; a = b; b = t; }
+    const int32_t old = atomicCAS(&parent[b], b, a);   // hook the larger root under the smaller
+    if (old == b) return;
+    b = old;
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_cc_init(int32_t* parent, uint32_t* cmin, int64_t nv) {
+  for (int64_t p = gtid(); p < nv; p += gstride()) { parent[p] = (int32_t)p; cmin[p] = 0xffffffffu; }
+}
+
+__global__ void __launch_bounds__(kBlock) k_cc_hook(const int32_t* __restrict__ tri, int64_t nt, int32_t* parent) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) {
+    uf_unite(parent, tri[3 * t], tri[3 * t + 1]);
+    uf_unite(parent, tri[3 * t], tri[3 * t + 2]);
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_cc_compress(int32_t* parent, int64_t nv) {
+  for (int64_t p = gtid(); p < nv; p += gstride()) parent[p] = uf_find(parent, (int32_t)p);
+}
+
+__global__ void __launch_bounds__(kBlock) k_cc_min(const int32_t* __restrict__ tri, int64_t nt,
+                                                   const int32_t* __restrict__ parent, uint32_t* cmin) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) atomicMin(&cmin[parent[tri[3 * t]]], (uint32_t)t);
+}
+
+__global__ void __launch_bounds__(kBlock) k_cc_flags(const int32_t* __restrict__ tri, int64_t nt,
+                                                     const int32_t* __restrict__ parent,
+                                                     const uint32_t* __restrict__ cmin, unsigned long long* flag,
+                                                     int32_t* reg, unsigned long long* best) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) {
+    flag[t] = cmin[parent[tri[3 * t]]] == (uint32_t)t ? 1ull : 0ull;
+    reg[t] = -1;
+    best[t] = kInf;
+  }
+}
+
+// wave 0 of every region: its lowest cell, at the region's number
+__global__ void __launch_bounds__(kBlock) k_cc_starts(const int32_t* __restrict__ tri, int64_t nt,
+                                                      const int32_t* __restrict__ parent,
+                                                      const uint32_t* __restrict__ cmin,
+                                                      const unsigned long long* __restrict__ regno, int32_t* seq,
+                                                      int32_t* reg, unsigned long long* best) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) {
+    if (cmin[parent[tri[3 * t]]] != (uint32_t)t) continue;
+    const int32_t r = (int32_t)regno[t];
+    seq[r] = (int32_t)t;
+    reg[t] = r;
+    best[t] = 0;
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_reset(int32_t* reg, unsigned long long* best, int64_t nt) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) { reg[t] = -1; best[t] = kInf; }
+}
+
+// ---- the waves ---------------------------------------------------------------------------------------------
+struct Lv {
+  const int32_t* tri;
+  const unsigned long long* lstart;
+  const int32_t* links;
+  const int64_t* seeds;
+  int32_t* seq;
+  int32_t* reg;
+  unsigned long long* best;
+  unsigned long long* loc1;
+  unsigned long long* loc2;
+  unsigned long long* btot;    // [0, kMaxGrid): appended entries per block; [kMaxGrid, 2 kMaxGrid): winners
+};
+
+// one wave; every block of a team computes the same record from the per-block totals
+struct State {
+  long long n;        // cells (or seeds) of the current wave
+  long long cur;      // its offset in seq (the seed wave: none)
+  long long base;     // first position of the wave's appended list; every earlier position is smaller
+  long long depth;    // waves that marked a cell
+  long long total;    // cells marked so far
+  long long seed;     // 1 while the current wave is the list of seeds
+};
+
+__device__ __forceinline__ int item_points(const Lv& P, const State& st, int64_t i, int32_t pts[3]) {
+  if (st.seed) {
+    const int64_t s = P.seeds[i];
+    pts[0] = (int32_t)s;
+    return s >= 0 ? 1 : 0;
+  }
+  const int32_t c = P.seq[st.cur + i];
+  pts[0] = P.tri[3 * c]; pts[1] = P.tri[3 * c + 1]; pts[2] = P.tri[3 * c + 2];
+  return 3;
+}
+
+// sum over blocks [0, b) and [0, nb) of btot[off + .], with the block's threads; s_r: 2 shared words
+__device__ __forceinline__ void block_prefix(const unsigned long long* btot, int b, int nb,
+                                             unsigned long long* s_r) {
+  if (threadIdx.x < 32) {
+    unsigned long long pre = 0, all = 0;
+    for (int k = threadIdx.x; k < nb; k += 32) {
+      const unsigned long long x = ((const volatile unsigned long long*)btot)[k];
+      all += x;
+      if (k < b) pre += x;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      pre += __shfl_xor_sync(0xffffffffu, pre, o);
+      all += __shfl_xor_sync(0xffffffffu, all, o);
+    }
+    if (threadIdx.x == 0) { s_r[0] = pre; s_r[1] = all; }
+  }
+  __syncthreads();
+}
+
+template <bool kGrid>
+__device__ __forceinline__ void team_sync(cg::grid_group& g) {
+  if (kGrid) g.sync(); else __syncthreads();
+}
+
+template <bool kGrid>
+__device__ void run_wave(const Lv& P, State& st, int b, int nb, cg::grid_group& g) {
+  __shared__ unsigned long long s_w[kBlock / 32];
+  __shared__ unsigned long long s_r[4];
+  const int64_t chunk = ceil_div64(st.n, nb);
+  const int64_t lo = (int64_t)b * chunk, hi = lo + chunk < st.n ? lo + chunk : st.n;
+  // 1. entries each item appends: the link lengths of its points
+  unsigned long long carry = 0;
+  for (int64_t t0 = lo; t0 < hi; t0 += kBlock) {
+    const int64_t i = t0 + threadIdx.x;
+    unsigned long long c = 0;
+    if (i < hi) {
+      int32_t pts[3];
+      const int np = item_points(P, st, i, pts);
+      for (int j = 0; j < np; ++j) c += P.lstart[pts[j] + 1] - P.lstart[pts[j]];
+    }
+    unsigned long long tot;
+    const unsigned long long ex = block_exscan<unsigned long long>(c, s_w, &tot);
+    if (i < hi) P.loc1[i] = carry + ex;
+    carry += tot;
+  }
+  if (threadIdx.x == 0) P.btot[b] = carry;
+  team_sync<kGrid>(g);
+  // 2. every unmarked candidate takes the lowest of its positions
+  block_prefix(P.btot, b, nb, s_r);
+  const unsigned long long pre1 = s_r[0] + (unsigned long long)st.base, all1 = s_r[1];
+  for (int64_t i = lo + threadIdx.x; i < hi; i += kBlock) {
+    unsigned long long q = pre1 + P.loc1[i];
+    int32_t pts[3];
+    const int np = item_points(P, st, i, pts);
+    for (int j = 0; j < np; ++j)
+      for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q) {
+        const int32_t d = P.links[k];
+        if (((volatile unsigned long long*)P.best)[d] >= (unsigned long long)st.base) atomicMin(&P.best[d], q);
+      }
+  }
+  team_sync<kGrid>(g);
+  // 3. winners per item: the entries at their cell's lowest position
+  carry = 0;
+  for (int64_t t0 = lo; t0 < hi; t0 += kBlock) {
+    const int64_t i = t0 + threadIdx.x;
+    unsigned long long c = 0;
+    if (i < hi) {
+      unsigned long long q = pre1 + P.loc1[i];
+      int32_t pts[3];
+      const int np = item_points(P, st, i, pts);
+      for (int j = 0; j < np; ++j)
+        for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q)
+          c += P.best[P.links[k]] == q;
+    }
+    unsigned long long tot;
+    const unsigned long long ex = block_exscan<unsigned long long>(c, s_w, &tot);
+    if (i < hi) P.loc2[i] = carry + ex;
+    carry += tot;
+  }
+  if (threadIdx.x == 0) P.btot[kMaxGrid + b] = carry;
+  team_sync<kGrid>(g);
+  // 4. the winners, in position order, are the next wave; they inherit the parent's region
+  block_prefix(P.btot + kMaxGrid, b, nb, s_r + 2);
+  const unsigned long long pre2 = s_r[2], all2 = s_r[3];
+  const long long out = st.seed ? 0 : st.cur + st.n;
+  for (int64_t i = lo + threadIdx.x; i < hi; i += kBlock) {
+    unsigned long long q = pre1 + P.loc1[i];
+    long long pos = out + (long long)(pre2 + P.loc2[i]);
+    int32_t pts[3];
+    const int np = item_points(P, st, i, pts);
+    const int32_t r = st.seed ? 0 : P.reg[P.seq[st.cur + i]];
+    for (int j = 0; j < np; ++j)
+      for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q) {
+        const int32_t d = P.links[k];
+        if (P.best[d] == q) { P.seq[pos++] = d; P.reg[d] = r; }
+      }
+  }
+  team_sync<kGrid>(g);
+  st.cur = out;
+  st.n = (long long)all2;
+  st.base += (long long)all1 + 1;
+  st.depth += all2 > 0;
+  st.total += (long long)all2;
+  st.seed = 0;
+}
+
+__device__ __forceinline__ void load_state(const long long* ctl, State& st) {
+  const volatile long long* c = ctl;
+  st.n = c[0]; st.cur = c[1]; st.base = c[2]; st.depth = c[3]; st.total = c[4]; st.seed = c[5];
+}
+
+__device__ __forceinline__ void store_state(long long* ctl, const State& st) {
+  ctl[0] = st.n; ctl[1] = st.cur; ctl[2] = st.base; ctl[3] = st.depth; ctl[4] = st.total; ctl[5] = st.seed;
+}
+
+// ctl[0..5]: the starting state; ctl[6..11] and ctl[0..5] alternate as the hand-over record of each
+// single-block stretch (a block may still read one record while block 0 writes the other)
+__global__ void __launch_bounds__(kBlock) k_conn_levels(Lv P, long long* ctl) {
+  cg::grid_group g = cg::this_grid();
+  State st;
+  load_state(ctl, st);
+  int flip = 1;
+  while (st.n > 0) {
+    if (st.n <= kSmall) {
+      if (blockIdx.x == 0) {
+        do run_wave<false>(P, st, 0, 1, g); while (st.n > 0 && st.n <= kSmall);
+        if (threadIdx.x == 0) store_state(ctl + 6 * flip, st);
+      }
+      g.sync();
+      load_state(ctl + 6 * flip, st);
+      flip ^= 1;
+      continue;
+    }
+    run_wave<true>(P, st, blockIdx.x, gridDim.x, g);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) { ctl[12] = st.depth; ctl[13] = st.total; }
+}
+
+// ---- ranks, PointMap, faces --------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kBlock) k_conn_sizes(const int32_t* __restrict__ seq, int64_t n,
+                                                       const int32_t* __restrict__ reg, unsigned long long* cnt,
+                                                       uint32_t* ka, uint32_t* va) {
+  for (int64_t g = gtid(); g < n; g += gstride()) {
+    const int32_t c = seq[g], r = reg[c];
+    atomicAdd(&cnt[r], 1ull);
+    ka[g] = (uint32_t)r;
+    va[g] = (uint32_t)c;
+  }
+}
+
+// the largest region: the highest size, ties to the lowest number
+__global__ void __launch_bounds__(kBlock) k_conn_largest(const unsigned long long* __restrict__ size, int64_t nr,
+                                                         unsigned long long* best) {
+  for (int64_t r = gtid(); r < nr; r += gstride()) atomicMax(best, (size[r] << 32) | (0xffffffffull - (uint64_t)r));
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_first_use(const int32_t* __restrict__ rank, int64_t n,
+                                                           const int32_t* __restrict__ tri, unsigned long long* fu) {
+  for (int64_t k = gtid(); k < n; k += gstride()) {
+    const int32_t c = rank[k];
+    for (int j = 0; j < 3; ++j) atomicMin(&fu[tri[3 * c + j]], (unsigned long long)(3 * k + j));
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_flags(const int32_t* __restrict__ rank, int64_t n,
+                                                       const int32_t* __restrict__ tri,
+                                                       const unsigned long long* __restrict__ fu,
+                                                       unsigned long long* cflag) {
+  for (int64_t k = gtid(); k < n; k += gstride()) {
+    const int32_t c = rank[k];
+    for (int j = 0; j < 3; ++j) cflag[3 * k + j] = fu[tri[3 * c + j]] == (unsigned long long)(3 * k + j);
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_pointmap(const int32_t* __restrict__ rank, int64_t n,
+                                                          const int32_t* __restrict__ tri,
+                                                          const unsigned long long* __restrict__ fu,
+                                                          const unsigned long long* __restrict__ cnum, int32_t* pmap,
+                                                          int32_t* inv) {
+  for (int64_t k = gtid(); k < n; k += gstride()) {
+    const int32_t c = rank[k];
+    for (int j = 0; j < 3; ++j) {
+      const int32_t p = tri[3 * c + j];
+      if (fu[p] != (unsigned long long)(3 * k + j)) continue;
+      const int32_t m = (int32_t)cnum[3 * k + j];
+      pmap[p] = m;
+      inv[m] = p;
+    }
+  }
+}
+
+// point offsets of the regions: the first-use count before each region's first rank
+__global__ void __launch_bounds__(kBlock) k_conn_ptoff(const unsigned long long* __restrict__ celloff, int64_t nr,
+                                                       const unsigned long long* __restrict__ cnum,
+                                                       unsigned long long* ptoff) {
+  for (int64_t r = gtid(); r <= nr; r += gstride()) ptoff[r] = cnum[3 * celloff[r]];
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_visited(const int32_t* __restrict__ reg, int64_t nt,
+                                                         unsigned long long* flag) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) flag[t] = reg[t] >= 0;
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_compact(const int32_t* __restrict__ reg, int64_t nt,
+                                                         const unsigned long long* __restrict__ idx, uint32_t* ka,
+                                                         uint32_t* va) {
+  for (int64_t t = gtid(); t < nt; t += gstride()) {
+    if (reg[t] < 0) continue;
+    ka[idx[t]] = (uint32_t)reg[t];
+    va[idx[t]] = (uint32_t)t;
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_emit_faces(const int32_t* __restrict__ cells, int64_t n,
+                                                            const int32_t* __restrict__ tri,
+                                                            const int32_t* __restrict__ pmap, int32_t* faces_out,
+                                                            int32_t* cell_ids) {
+  for (int64_t i = gtid(); i < n; i += gstride()) {
+    const int32_t c = cells[i];
+    cell_ids[i] = c;
+    for (int j = 0; j < 3; ++j) faces_out[3 * i + j] = pmap[tri[3 * c + j]];
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_conn_emit_points(const float* __restrict__ verts,
+                                                             const int32_t* __restrict__ inv, int64_t n,
+                                                             float* verts_out, int32_t* point_ids) {
+  for (int64_t m = gtid(); m < n; m += gstride()) {
+    const int32_t p = inv[m];
+    point_ids[m] = p;
+    verts_out[3 * m] = verts[3 * (int64_t)p];
+    verts_out[3 * m + 1] = verts[3 * (int64_t)p + 1];
+    verts_out[3 * m + 2] = verts[3 * (int64_t)p + 2];
+  }
+}
+
+__global__ void k_conn_offsets(const unsigned long long* __restrict__ celloff,
+                               const unsigned long long* __restrict__ ptoff, int64_t nr, int64_t* cell_off,
+                               int64_t* point_off) {
+  for (int64_t r = gtid(); r <= nr; r += gstride()) {
+    cell_off[r] = (int64_t)celloff[r];
+    point_off[r] = (int64_t)ptoff[r];
+  }
+}
+
+int check_args(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+               int64_t nseeds, const char* what) {
+  B2V_REQUIRE(nv >= 0 && nv <= 0x7fffffffLL && nt >= 0 && nt <= 0x7fffffffLL, B2V_ERR_ARG,
+              "%s: need V < 2^31 and T < 2^31", what);
+  B2V_REQUIRE(face_cols == 3 || face_cols == 4, B2V_ERR_ARG, "%s: faces must be [T,3] or [T,4]", what);
+  B2V_REQUIRE(faces_i64 == 0 || faces_i64 == 1, B2V_ERR_ARG, "%s: faces_i64 must be 0 or 1", what);
+  B2V_REQUIRE(nt == 0 || nv > 0, B2V_ERR_ARG, "%s: faces without vertices", what);
+  B2V_REQUIRE((nv == 0 || verts) && (nt == 0 || faces), B2V_ERR_ARG, "%s: null device pointer", what);
+  B2V_REQUIRE(nseeds >= 0, B2V_ERR_ARG, "%s: negative seed count", what);
+  return B2V_OK;
+}
+
+}  // namespace
+
+extern "C" int64_t b2v_conn_workspace_bytes(int64_t nv, int64_t nt, int64_t nseeds) {
+  if (nv < 0 || nt < 0 || nseeds < 0) return -1;
+  return (int64_t)carve(nullptr, nv, nt, nseeds).bytes;
+}
+
+extern "C" int b2v_conn_layout(int64_t nv, int64_t nt, int64_t nseeds, int64_t* layout_out) {
+  B2V_REQUIRE(nv >= 0 && nt >= 0 && nseeds >= 0 && layout_out, B2V_ERR_ARG, "conn_layout: bad arguments");
+  const ConnWs w = carve(nullptr, nv, nt, nseeds);
+  layout_out[0] = (int64_t)((char*)w.reg - (char*)nullptr);    // int32 [T]: region of each cell, -1 unvisited
+  layout_out[1] = (int64_t)((char*)w.pmap - (char*)nullptr);   // int32 [V]: PointMap, -1 unnumbered
+  layout_out[2] = (int64_t)((char*)w.seq - (char*)nullptr);    // int32 [C]: visited cells in wave order
+  layout_out[3] = (int64_t)((char*)w.rank - (char*)nullptr);   // int32 [C]: visited cells, region-major
+  layout_out[4] = (int64_t)((char*)w.links - (char*)nullptr);  // int32 [3T]: point -> cell links
+  layout_out[5] = (int64_t)((char*)w.lstart - (char*)nullptr); // uint64 [V + 1]: their offsets
+  return B2V_OK;
+}
+
+extern "C" int b2v_conn_count(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols,
+                              int faces_i64, int seeded, const int64_t* seeds_host, int64_t nseeds, void* workspace,
+                              void* stream, int64_t* counts_host) {
+  if (int rc = check_args(verts, nv, faces, nt, face_cols, faces_i64, seeded ? nseeds : 0, "conn_count")) return rc;
+  B2V_REQUIRE(workspace && counts_host && (!seeded || nseeds == 0 || seeds_host), B2V_ERR_ARG,
+              "conn_count: null argument");
+  if (seeded)
+    for (int64_t i = 0; i < nseeds; ++i)
+      B2V_REQUIRE(seeds_host[i] < nv, B2V_ERR_ARG, "connectivity: seed %lld is not a point id (V = %lld)",
+                  (long long)seeds_host[i], (long long)nv);
+  if (!seeded) nseeds = 0;
+  for (int k = 0; k < 4; ++k) counts_host[k] = 0;
+  counts_host[4] = -1;
+  if (seeded) counts_host[0] = 1;
+  if (nt == 0) return B2V_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  ConnWs w = carve(workspace, nv, nt, nseeds);
+  const int64_t C3 = 3 * nt;
+  B2V_CUDA(cudaMemsetAsync(w.status, 0, 16, s));
+  B2V_CUDA(cudaMemsetAsync(w.totals, 0, 64, s));
+  B2V_CUDA(cudaMemsetAsync(w.lstart, 0, (size_t)(nv + 1) * 8, s));
+
+  // faces, link counts and offsets, the links themselves (corners stably sorted by point)
+  k_conn_load<<<grid_for(nt), kBlock, 0, s>>>(faces, nt, face_cols, faces_i64, nv, w.tri, w.lstart, w.ka, w.va,
+                                              w.status);
+  if (int rc = b2v_check_launch("k_conn_load")) return rc;
+  uint32_t status = 0;
+  B2V_CUDA(cudaMemcpyAsync(&status, w.status, 4, cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaStreamSynchronize(s));
+  B2V_REQUIRE(!(status & ST_BAD_FACE), B2V_ERR_ARG,
+              "connectivity: a face has an index outside [0, V) (or a leading entry other than 3)");
+  if (int rc = scan(w.lstart, nv + 1, w.scratch, nullptr, s)) return rc;
+  uint32_t* lv = nullptr;
+  if (int rc = sort_pairs(w, C3, bits_for(nv - 1), &lv, s)) return rc;
+  k_copy_i32<<<grid_for(C3), kBlock, 0, s>>>(lv, C3, w.links);
+  if (int rc = b2v_check_launch("k_copy_i32")) return rc;
+
+  // wave 0 and the starting state
+  long long st[6] = {0, 0, 1, 0, 0, 0};
+  if (seeded) {
+    k_conn_reset<<<grid_for(nt), kBlock, 0, s>>>(w.reg, w.best, nt);
+    if (int rc = b2v_check_launch("k_conn_reset")) return rc;
+    if (nseeds) B2V_CUDA(cudaMemcpyAsync(w.seeds, seeds_host, (size_t)nseeds * 8, cudaMemcpyHostToDevice, s));
+    st[0] = nseeds;
+    st[5] = 1;
+  } else {
+    k_cc_init<<<grid_for(nv), kBlock, 0, s>>>(w.parent, w.cmin, nv);
+    if (int rc = b2v_check_launch("k_cc_init")) return rc;
+    k_cc_hook<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent);
+    if (int rc = b2v_check_launch("k_cc_hook")) return rc;
+    k_cc_compress<<<grid_for(nv), kBlock, 0, s>>>(w.parent, nv);
+    if (int rc = b2v_check_launch("k_cc_compress")) return rc;
+    k_cc_min<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin);
+    if (int rc = b2v_check_launch("k_cc_min")) return rc;
+    k_cc_flags<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.reg, w.best);
+    if (int rc = b2v_check_launch("k_cc_flags")) return rc;
+    if (int rc = scan(w.tflag, nt, w.scratch, w.totals, s)) return rc;
+    k_cc_starts<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.seq, w.reg, w.best);
+    if (int rc = b2v_check_launch("k_cc_starts")) return rc;
+    unsigned long long nreg = 0;
+    B2V_CUDA(cudaMemcpyAsync(&nreg, w.totals, 8, cudaMemcpyDeviceToHost, s));
+    B2V_CUDA(cudaStreamSynchronize(s));
+    st[0] = (long long)nreg;
+    st[3] = nreg > 0;
+    st[4] = (long long)nreg;
+  }
+  B2V_CUDA(cudaMemcpyAsync(w.ctl, st, sizeof(st), cudaMemcpyHostToDevice, s));
+
+  // every wave of every region: one persistent cooperative launch
+  int per_sm = 0;
+  B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_conn_levels, kBlock, 0));
+  B2V_REQUIRE(per_sm >= 1, B2V_ERR_CUDA, "connectivity: the wave kernel does not fit on an SM");
+  if (per_sm > 2) per_sm = 2;
+  int grid = per_sm * b2v_sm_count();
+  if (grid > kMaxGrid) grid = kMaxGrid;
+  Lv P{w.tri, w.lstart, w.links, w.seeds, w.seq, w.reg, w.best, w.loc1, w.loc2, w.btot};
+  long long* ctl = w.ctl;
+  void* args[] = {&P, &ctl};
+  B2V_CUDA(cudaLaunchCooperativeKernel((const void*)k_conn_levels, dim3(grid), dim3(kBlock), args, 0, s));
+  if (int rc = b2v_check_launch("k_conn_levels")) return rc;
+  long long res[2] = {0, 0};
+  B2V_CUDA(cudaMemcpyAsync(res, ctl + 12, sizeof(res), cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaStreamSynchronize(s));
+  const long long depth = res[0], ncells = res[1];
+  const long long nreg = seeded ? 1 : st[0];
+
+  // region sizes and offsets, the largest region, the region-major ranks
+  B2V_CUDA(cudaMemsetAsync(w.celloff, 0, (size_t)(nreg + 1) * 8, s));
+  B2V_CUDA(cudaMemsetAsync(w.fu, 0xff, (size_t)nv * 8, s));
+  B2V_CUDA(cudaMemsetAsync(w.pmap, 0xff, (size_t)nv * 4, s));
+  if (ncells > 0) {
+    k_conn_sizes<<<grid_for(ncells), kBlock, 0, s>>>(w.seq, ncells, w.reg, w.celloff, w.ka, w.va);
+    if (int rc = b2v_check_launch("k_conn_sizes")) return rc;
+    k_conn_largest<<<grid_for(nreg), kBlock, 0, s>>>(w.celloff, nreg, w.totals + 1);
+    if (int rc = b2v_check_launch("k_conn_largest")) return rc;
+  }
+  if (int rc = scan(w.celloff, nreg + 1, w.scratch, nullptr, s)) return rc;
+  uint32_t* rv = nullptr;
+  if (int rc = sort_pairs(w, ncells, bits_for(nreg - 1), &rv, s)) return rc;
+  if (ncells > 0) {
+    k_copy_i32<<<grid_for(ncells), kBlock, 0, s>>>(rv, ncells, w.rank);
+    if (int rc = b2v_check_launch("k_copy_i32")) return rc;
+    // PointMap: first use over (rank, j), numbered by a scan of the first-use flags
+    k_conn_first_use<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu);
+    if (int rc = b2v_check_launch("k_conn_first_use")) return rc;
+    k_conn_flags<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag);
+    if (int rc = b2v_check_launch("k_conn_flags")) return rc;
+  }
+  B2V_CUDA(cudaMemsetAsync(w.cflag + 3 * ncells, 0, 8, s));
+  if (int rc = scan(w.cflag, 3 * ncells + 1, w.scratch, w.totals + 2, s)) return rc;
+  if (ncells > 0) {
+    k_conn_pointmap<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag, w.pmap, w.inv);
+    if (int rc = b2v_check_launch("k_conn_pointmap")) return rc;
+  }
+  k_conn_ptoff<<<grid_for(nreg + 1), kBlock, 0, s>>>(w.celloff, nreg, w.cflag, w.ptoff);
+  if (int rc = b2v_check_launch("k_conn_ptoff")) return rc;
+
+  // the visited cells in ascending id, stably grouped by region
+  k_conn_visited<<<grid_for(nt), kBlock, 0, s>>>(w.reg, nt, w.tflag);
+  if (int rc = b2v_check_launch("k_conn_visited")) return rc;
+  if (int rc = scan(w.tflag, nt, w.scratch, nullptr, s)) return rc;
+  k_conn_compact<<<grid_for(nt), kBlock, 0, s>>>(w.reg, nt, w.tflag, w.ka, w.va);
+  if (int rc = b2v_check_launch("k_conn_compact")) return rc;
+  uint32_t* cv = nullptr;
+  if (int rc = sort_pairs(w, ncells, bits_for(nreg - 1), &cv, s)) return rc;
+  if (ncells > 0) {
+    k_copy_i32<<<grid_for(ncells), kBlock, 0, s>>>(cv, ncells, w.cells);
+    if (int rc = b2v_check_launch("k_copy_i32")) return rc;
+  }
+
+  unsigned long long tot[3] = {0, 0, 0};
+  B2V_CUDA(cudaMemcpyAsync(tot, w.totals, sizeof(tot), cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaStreamSynchronize(s));
+  counts_host[0] = nreg;
+  counts_host[1] = (int64_t)tot[2];
+  counts_host[2] = ncells;
+  counts_host[3] = depth;
+  counts_host[4] = ncells > 0 ? (int64_t)(0xffffffffull - (tot[1] & 0xffffffffull)) : -1;
+  return B2V_OK;
+}
+
+extern "C" int b2v_conn_emit(const float* verts, int64_t nv, int64_t nt, int64_t nseeds, const int64_t* counts_host,
+                             void* workspace, float* verts_out, int32_t* point_ids, int32_t* faces_out,
+                             int32_t* cell_ids, int64_t* point_offsets, int64_t* cell_offsets, void* stream) {
+  B2V_REQUIRE(nv >= 0 && nt >= 0 && nseeds >= 0 && counts_host && workspace, B2V_ERR_ARG, "conn_emit: bad arguments");
+  const int64_t nreg = counts_host[0], npts = counts_host[1], ncells = counts_host[2];
+  B2V_REQUIRE(nreg >= 0 && nreg <= (nt > 1 ? nt : 1) && npts >= 0 && npts <= nv && ncells >= 0 && ncells <= nt,
+              B2V_ERR_ARG, "conn_emit: counts do not come from b2v_conn_count on this mesh");
+  B2V_REQUIRE((npts == 0 || (verts && verts_out && point_ids)) && (ncells == 0 || (faces_out && cell_ids)) &&
+                  (point_offsets && cell_offsets),
+              B2V_ERR_ARG, "conn_emit: null output");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (nt == 0) {
+    B2V_CUDA(cudaMemsetAsync(point_offsets, 0, (size_t)(nreg + 1) * 8, s));
+    B2V_CUDA(cudaMemsetAsync(cell_offsets, 0, (size_t)(nreg + 1) * 8, s));
+    return B2V_OK;
+  }
+  const ConnWs w = carve(workspace, nv, nt, nseeds);
+  if (npts > 0) {
+    k_conn_emit_points<<<grid_for(npts), kBlock, 0, s>>>(verts, w.inv, npts, verts_out, point_ids);
+    if (int rc = b2v_check_launch("k_conn_emit_points")) return rc;
+  }
+  if (ncells > 0) {
+    k_conn_emit_faces<<<grid_for(ncells), kBlock, 0, s>>>(w.cells, ncells, w.tri, w.pmap, faces_out, cell_ids);
+    if (int rc = b2v_check_launch("k_conn_emit_faces")) return rc;
+  }
+  k_conn_offsets<<<grid_for(nreg + 1), kBlock, 0, s>>>(w.celloff, w.ptoff, nreg, cell_offsets, point_offsets);
+  return b2v_check_launch("k_conn_offsets");
+}
