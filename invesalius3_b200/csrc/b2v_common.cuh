@@ -98,3 +98,76 @@ __device__ __forceinline__ uint32_t nonzero_flags_u8x4(uint32_t x) {
 }
 
 __host__ __device__ __forceinline__ int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// ---- launch shapes and workspace layout -----------------------------------------
+// Blocks for a grid-stride launch over `items` at `per_block` items a block: enough to cover them once,
+// at most per_sm blocks per SM, and never 0 (a launch of 0 blocks fails).
+static inline int b2v_grid(int64_t items, int per_block, int per_sm) {
+  int64_t blocks = ceil_div64(items, per_block);
+  const int64_t cap = (int64_t)b2v_sm_count() * per_sm;
+  if (blocks > cap) blocks = cap;
+  return (int)(blocks < 1 ? 1 : blocks);
+}
+
+// workspace buffers start on 256-byte boundaries
+static inline int64_t align256(int64_t bytes) { return (bytes + 255) & ~(int64_t)255; }
+
+__device__ __forceinline__ int64_t gtid() { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; }
+__device__ __forceinline__ int64_t gstride() { return (int64_t)gridDim.x * blockDim.x; }
+
+// Block-wide exclusive scan: returns x's prefix and stores the block total. Every thread of the block calls
+// it; blockDim.x is a multiple of 32, and s_w holds blockDim.x / 32 words.
+template <typename T>
+__device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  T inc = x;
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  if (lane == 31) s_w[wid] = inc;
+  __syncthreads();
+  if (wid == 0) {
+    const int nw = blockDim.x >> 5;
+    T v = lane < nw ? s_w[lane] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const T y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += y;
+    }
+    if (lane < nw) s_w[lane] = v;
+  }
+  __syncthreads();
+  const T base = wid ? s_w[wid - 1] : 0;
+  *total = s_w[(blockDim.x >> 5) - 1];
+  __syncthreads();
+  return base + inc - x;
+}
+
+// ---- triangle faces ---------------------------------------------------------------
+// int32 or int64 ids, [T,3] or [T,4] with a leading 3 (the Mesh form), every id in [0, nv)
+struct Faces {
+  const void* p;
+  int64_t nt;
+  int cols;    // 3, or 4 with a leading 3
+  int i64;
+  int64_t nv;
+};
+
+enum : uint32_t { ST_BAD_FACE = 1u };   // status bit: some face failed load_face
+
+// the three vertex ids of face t; false when the face is malformed (an index outside [0, nv) or a leading
+// entry other than 3 in the [T, 4] form)
+__device__ __forceinline__ bool load_face(const Faces& F, int64_t t, int64_t v[3]) {
+  const int64_t base = t * F.cols;
+  const int off = F.cols == 4 ? 1 : 0;
+  if (F.i64) {
+    const int64_t* f = (const int64_t*)F.p + base;
+    if (off && f[0] != 3) return false;
+    v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
+  } else {
+    const int32_t* f = (const int32_t*)F.p + base;
+    if (off && f[0] != 3) return false;
+    v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
+  }
+  return v[0] >= 0 && v[0] < F.nv && v[1] >= 0 && v[1] < F.nv && v[2] >= 0 && v[2] < F.nv;
+}

@@ -40,8 +40,6 @@ constexpr int kMaxGrid = 1024;                     // blocks of the persistent l
 constexpr int64_t kSmall = 2048;                   // waves this small run in one block
 constexpr unsigned long long kInf = ~0ull;
 
-enum : uint32_t { ST_BAD_FACE = 1u };
-
 struct ConnWs {
   long long* ctl;                  // [0..15]: two state records for the persistent launch, then results
   uint32_t* status;
@@ -73,15 +71,13 @@ struct ConnWs {
   size_t bytes;
 };
 
-inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int64_t scan_blocks(int64_t n) { return ceil_div64(n > 0 ? n : 1, kScanTile); }
 
 ConnWs carve(void* base, int64_t nv, int64_t nt, int64_t nseeds) {
   ConnWs w;
   char* p = (char*)base;
   size_t o = 0;
-  auto take = [&](size_t n) { char* r = p + o; o += al(n); return r; };
+  auto take = [&](size_t n) { char* r = p + o; o += align256(n); return r; };
   const size_t V = (size_t)nv, T = (size_t)nt, C3 = 3 * T;
   const size_t items = T > (size_t)nseeds ? T : (size_t)nseeds;
   w.nb3 = ceil_div64((int64_t)(C3 > 0 ? C3 : 1), kBlock);
@@ -121,43 +117,6 @@ ConnWs carve(void* base, int64_t nv, int64_t nt, int64_t nseeds) {
   w.ptoff = (unsigned long long*)take((T + 2) * 8);
   w.bytes = o;
   return w;
-}
-
-__device__ __forceinline__ int64_t gtid() { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; }
-__device__ __forceinline__ int64_t gstride() { return (int64_t)gridDim.x * blockDim.x; }
-
-unsigned grid_for(int64_t n, int per_sm = 16) {
-  int64_t b = ceil_div64(n, kBlock);
-  const int64_t cap = (int64_t)b2v_sm_count() * per_sm;
-  if (b > cap) b = cap;
-  return (unsigned)(b < 1 ? 1 : b);
-}
-
-// block-wide exclusive scan (kBlock threads); returns the prefix and the block total
-template <typename T>
-__device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  T inc = x;
-  for (int o = 1; o < 32; o <<= 1) {
-    const T y = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += y;
-  }
-  if (lane == 31) s_w[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    const int nw = blockDim.x >> 5;
-    T v = lane < nw ? s_w[lane] : 0;
-    for (int o = 1; o < 32; o <<= 1) {
-      const T y = __shfl_up_sync(0xffffffffu, v, o);
-      if (lane >= o) v += y;
-    }
-    if (lane < nw) s_w[lane] = v;
-  }
-  __syncthreads();
-  const T base = wid ? s_w[wid - 1] : 0;
-  *total = s_w[(blockDim.x >> 5) - 1];
-  __syncthreads();
-  return base + inc - x;
 }
 
 // ---- device-wide exclusive scan of uint64 in place (tiles of kScanTile, then the tile sums) ----------------
@@ -271,24 +230,11 @@ int bits_for(int64_t max_key) {
 }
 
 // ---- faces and links -------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBlock) k_conn_load(const void* faces, int64_t nt, int cols, int i64, int64_t nv,
-                                                     int32_t* __restrict__ tri, unsigned long long* deg,
+__global__ void __launch_bounds__(kBlock) k_conn_load(Faces F, int32_t* __restrict__ tri, unsigned long long* deg,
                                                      uint32_t* ka, uint32_t* va, uint32_t* status) {
-  for (int64_t t = gtid(); t < nt; t += gstride()) {
-    const int off = cols == 4 ? 1 : 0;
-    int64_t v[3], lead;
-    if (i64) {
-      const int64_t* f = (const int64_t*)faces + t * cols;
-      lead = off ? f[0] : 3;
-      v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
-    } else {
-      const int32_t* f = (const int32_t*)faces + t * cols;
-      lead = off ? f[0] : 3;
-      v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
-    }
-    bool ok = lead == 3;
-    for (int j = 0; j < 3; ++j) ok = ok && v[j] >= 0 && v[j] < nv;
-    if (!ok) {
+  for (int64_t t = gtid(); t < F.nt; t += gstride()) {
+    int64_t v[3];
+    if (!load_face(F, t, v)) {
       atomicOr(status, ST_BAD_FACE);
       v[0] = v[1] = v[2] = 0;
     }
@@ -709,8 +655,8 @@ extern "C" int b2v_conn_count(const float* verts, int64_t nv, const void* faces,
   B2V_CUDA(cudaMemsetAsync(w.lstart, 0, (size_t)(nv + 1) * 8, s));
 
   // faces, link counts and offsets, the links themselves (corners stably sorted by point)
-  k_conn_load<<<grid_for(nt), kBlock, 0, s>>>(faces, nt, face_cols, faces_i64, nv, w.tri, w.lstart, w.ka, w.va,
-                                              w.status);
+  const Faces F{faces, nt, face_cols, faces_i64, nv};
+  k_conn_load<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(F, w.tri, w.lstart, w.ka, w.va, w.status);
   if (int rc = b2v_check_launch("k_conn_load")) return rc;
   uint32_t status = 0;
   B2V_CUDA(cudaMemcpyAsync(&status, w.status, 4, cudaMemcpyDeviceToHost, s));
@@ -720,30 +666,30 @@ extern "C" int b2v_conn_count(const float* verts, int64_t nv, const void* faces,
   if (int rc = scan(w.lstart, nv + 1, w.scratch, nullptr, s)) return rc;
   uint32_t* lv = nullptr;
   if (int rc = sort_pairs(w, C3, bits_for(nv - 1), &lv, s)) return rc;
-  k_copy_i32<<<grid_for(C3), kBlock, 0, s>>>(lv, C3, w.links);
+  k_copy_i32<<<b2v_grid(C3, kBlock, 16), kBlock, 0, s>>>(lv, C3, w.links);
   if (int rc = b2v_check_launch("k_copy_i32")) return rc;
 
   // wave 0 and the starting state
   long long st[6] = {0, 0, 1, 0, 0, 0};
   if (seeded) {
-    k_conn_reset<<<grid_for(nt), kBlock, 0, s>>>(w.reg, w.best, nt);
+    k_conn_reset<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.reg, w.best, nt);
     if (int rc = b2v_check_launch("k_conn_reset")) return rc;
     if (nseeds) B2V_CUDA(cudaMemcpyAsync(w.seeds, seeds_host, (size_t)nseeds * 8, cudaMemcpyHostToDevice, s));
     st[0] = nseeds;
     st[5] = 1;
   } else {
-    k_cc_init<<<grid_for(nv), kBlock, 0, s>>>(w.parent, w.cmin, nv);
+    k_cc_init<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(w.parent, w.cmin, nv);
     if (int rc = b2v_check_launch("k_cc_init")) return rc;
-    k_cc_hook<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent);
+    k_cc_hook<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.tri, nt, w.parent);
     if (int rc = b2v_check_launch("k_cc_hook")) return rc;
-    k_cc_compress<<<grid_for(nv), kBlock, 0, s>>>(w.parent, nv);
+    k_cc_compress<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(w.parent, nv);
     if (int rc = b2v_check_launch("k_cc_compress")) return rc;
-    k_cc_min<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin);
+    k_cc_min<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin);
     if (int rc = b2v_check_launch("k_cc_min")) return rc;
-    k_cc_flags<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.reg, w.best);
+    k_cc_flags<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.reg, w.best);
     if (int rc = b2v_check_launch("k_cc_flags")) return rc;
     if (int rc = scan(w.tflag, nt, w.scratch, w.totals, s)) return rc;
-    k_cc_starts<<<grid_for(nt), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.seq, w.reg, w.best);
+    k_cc_starts<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.tri, nt, w.parent, w.cmin, w.tflag, w.seq, w.reg, w.best);
     if (int rc = b2v_check_launch("k_cc_starts")) return rc;
     unsigned long long nreg = 0;
     B2V_CUDA(cudaMemcpyAsync(&nreg, w.totals, 8, cudaMemcpyDeviceToHost, s));
@@ -777,42 +723,43 @@ extern "C" int b2v_conn_count(const float* verts, int64_t nv, const void* faces,
   B2V_CUDA(cudaMemsetAsync(w.fu, 0xff, (size_t)nv * 8, s));
   B2V_CUDA(cudaMemsetAsync(w.pmap, 0xff, (size_t)nv * 4, s));
   if (ncells > 0) {
-    k_conn_sizes<<<grid_for(ncells), kBlock, 0, s>>>(w.seq, ncells, w.reg, w.celloff, w.ka, w.va);
+    k_conn_sizes<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(w.seq, ncells, w.reg, w.celloff, w.ka, w.va);
     if (int rc = b2v_check_launch("k_conn_sizes")) return rc;
-    k_conn_largest<<<grid_for(nreg), kBlock, 0, s>>>(w.celloff, nreg, w.totals + 1);
+    k_conn_largest<<<b2v_grid(nreg, kBlock, 16), kBlock, 0, s>>>(w.celloff, nreg, w.totals + 1);
     if (int rc = b2v_check_launch("k_conn_largest")) return rc;
   }
   if (int rc = scan(w.celloff, nreg + 1, w.scratch, nullptr, s)) return rc;
   uint32_t* rv = nullptr;
   if (int rc = sort_pairs(w, ncells, bits_for(nreg - 1), &rv, s)) return rc;
   if (ncells > 0) {
-    k_copy_i32<<<grid_for(ncells), kBlock, 0, s>>>(rv, ncells, w.rank);
+    k_copy_i32<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(rv, ncells, w.rank);
     if (int rc = b2v_check_launch("k_copy_i32")) return rc;
     // PointMap: first use over (rank, j), numbered by a scan of the first-use flags
-    k_conn_first_use<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu);
+    k_conn_first_use<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu);
     if (int rc = b2v_check_launch("k_conn_first_use")) return rc;
-    k_conn_flags<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag);
+    k_conn_flags<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag);
     if (int rc = b2v_check_launch("k_conn_flags")) return rc;
   }
   B2V_CUDA(cudaMemsetAsync(w.cflag + 3 * ncells, 0, 8, s));
   if (int rc = scan(w.cflag, 3 * ncells + 1, w.scratch, w.totals + 2, s)) return rc;
   if (ncells > 0) {
-    k_conn_pointmap<<<grid_for(ncells), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag, w.pmap, w.inv);
+    k_conn_pointmap<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(w.rank, ncells, w.tri, w.fu, w.cflag, w.pmap,
+                                                                    w.inv);
     if (int rc = b2v_check_launch("k_conn_pointmap")) return rc;
   }
-  k_conn_ptoff<<<grid_for(nreg + 1), kBlock, 0, s>>>(w.celloff, nreg, w.cflag, w.ptoff);
+  k_conn_ptoff<<<b2v_grid(nreg + 1, kBlock, 16), kBlock, 0, s>>>(w.celloff, nreg, w.cflag, w.ptoff);
   if (int rc = b2v_check_launch("k_conn_ptoff")) return rc;
 
   // the visited cells in ascending id, stably grouped by region
-  k_conn_visited<<<grid_for(nt), kBlock, 0, s>>>(w.reg, nt, w.tflag);
+  k_conn_visited<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.reg, nt, w.tflag);
   if (int rc = b2v_check_launch("k_conn_visited")) return rc;
   if (int rc = scan(w.tflag, nt, w.scratch, nullptr, s)) return rc;
-  k_conn_compact<<<grid_for(nt), kBlock, 0, s>>>(w.reg, nt, w.tflag, w.ka, w.va);
+  k_conn_compact<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(w.reg, nt, w.tflag, w.ka, w.va);
   if (int rc = b2v_check_launch("k_conn_compact")) return rc;
   uint32_t* cv = nullptr;
   if (int rc = sort_pairs(w, ncells, bits_for(nreg - 1), &cv, s)) return rc;
   if (ncells > 0) {
-    k_copy_i32<<<grid_for(ncells), kBlock, 0, s>>>(cv, ncells, w.cells);
+    k_copy_i32<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(cv, ncells, w.cells);
     if (int rc = b2v_check_launch("k_copy_i32")) return rc;
   }
 
@@ -845,13 +792,15 @@ extern "C" int b2v_conn_emit(const float* verts, int64_t nv, int64_t nt, int64_t
   }
   const ConnWs w = carve(workspace, nv, nt, nseeds);
   if (npts > 0) {
-    k_conn_emit_points<<<grid_for(npts), kBlock, 0, s>>>(verts, w.inv, npts, verts_out, point_ids);
+    k_conn_emit_points<<<b2v_grid(npts, kBlock, 16), kBlock, 0, s>>>(verts, w.inv, npts, verts_out, point_ids);
     if (int rc = b2v_check_launch("k_conn_emit_points")) return rc;
   }
   if (ncells > 0) {
-    k_conn_emit_faces<<<grid_for(ncells), kBlock, 0, s>>>(w.cells, ncells, w.tri, w.pmap, faces_out, cell_ids);
+    k_conn_emit_faces<<<b2v_grid(ncells, kBlock, 16), kBlock, 0, s>>>(w.cells, ncells, w.tri, w.pmap, faces_out,
+                                                                      cell_ids);
     if (int rc = b2v_check_launch("k_conn_emit_faces")) return rc;
   }
-  k_conn_offsets<<<grid_for(nreg + 1), kBlock, 0, s>>>(w.celloff, w.ptoff, nreg, cell_offsets, point_offsets);
+  k_conn_offsets<<<b2v_grid(nreg + 1, kBlock, 16), kBlock, 0, s>>>(w.celloff, w.ptoff, nreg, cell_offsets,
+                                                                   point_offsets);
   return b2v_check_launch("k_conn_offsets");
 }

@@ -219,13 +219,6 @@ bool brush_box(int64_t dz, int64_t dy, int64_t dx, const double* sp, const doubl
          brush_axis(c[0], r, sp[0], dx, &box[2], &box[5]);
 }
 
-int grid_for(long long work, long long per_block_cap) {
-  long long blocks = ceil_div64(work, 256);
-  const long long cap = (long long)b2v_sm_count() * per_block_cap;
-  if (blocks > cap) blocks = cap;
-  return (int)(blocks < 1 ? 1 : blocks);
-}
-
 }  // namespace
 
 extern "C" int b2v_polygon2mask(const double* polygon_host, int64_t n, int64_t w, int64_t h, uint8_t* out,
@@ -279,7 +272,7 @@ extern "C" int b2v_mask_cut(uint8_t* out, int64_t dz, int64_t dy, int64_t dx, co
   P.dy = dy; P.dx = dx; P.h = h; P.w = w; P.n = n;
   P.edit_mode = edit_mode;
   cudaStream_t s = (cudaStream_t)stream;
-  k_mask_cut<<<grid_for(ceil_div64(n, 16), 64), 256, 0, s>>>(out, filter, P);
+  k_mask_cut<<<b2v_grid(ceil_div64(n, 16), 256, 64), 256, 0, s>>>(out, filter, P);
   return b2v_check_launch("k_mask_cut");
 }
 
@@ -316,6 +309,6 @@ extern "C" int b2v_brush_mask(uint8_t* out, const uint8_t* orig, int64_t dz, int
   P.oz = oz; P.oy = oy; P.ox = ox; P.row_pitch = row_pitch; P.plane_pitch = plane_pitch;
   P.edit_mode = edit_mode;
   cudaStream_t s = (cudaStream_t)stream;
-  k_brush_mask<<<grid_for(P.bz * P.by * P.bx, 16), 256, 0, s>>>(out, orig, P);
+  k_brush_mask<<<b2v_grid(P.bz * P.by * P.bx, 256, 16), 256, 0, s>>>(out, orig, P);
   return b2v_check_launch("k_brush_mask");
 }

@@ -14,14 +14,6 @@
 
 namespace {
 
-int fgrid(long long n, int per = 256) {
-  long long blocks = ceil_div64(n, per);
-  long long cap = (long long)b2v_sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 __device__ __forceinline__ long long reflect_idx(long long i, long long n) {   // scipy mode='reflect': (d c b a | a b c d | d c b a)
   if (n == 1) return 0;
   const long long period = 2 * n;
@@ -368,7 +360,7 @@ __global__ void __launch_bounds__(1024) k_histogram_i16(const int16_t* __restric
 
 extern "C" int b2v_boolean_op(const uint8_t* m1, const uint8_t* m2, int64_t n, int op, uint8_t* out, void* stream) {
   B2V_REQUIRE(m1 && m2 && out && n > 0 && op >= 0 && op <= 3, B2V_ERR_ARG, "boolean_op: bad arguments");
-  k_boolean_op<<<fgrid(n, 1024), 256, 0, (cudaStream_t)stream>>>(m1, m2, n, op, out);
+  k_boolean_op<<<b2v_grid(n, 1024, 32), 256, 0, (cudaStream_t)stream>>>(m1, m2, n, op, out);
   return b2v_check_launch("k_boolean_op");
 }
 
@@ -378,8 +370,8 @@ extern "C" int b2v_convolve_non_zero(const double* volume, int64_t sz, int64_t s
               "convolve_non_zero: bad arguments");
   B2V_REQUIRE(sz < (1ll << 30) && sy < (1ll << 30) && sx < (1ll << 30) && skz * sky * skx < (1ll << 20), B2V_ERR_ARG,
               "convolve_non_zero: shape too large");
-  k_convolve_non_zero<<<fgrid(sz * sy * sx), 256, 0, (cudaStream_t)stream>>>(volume, (int)sz, (int)sy, (int)sx, kernel_dev,
-                                                                             (int)skz, (int)sky, (int)skx, cval, out);
+  k_convolve_non_zero<<<b2v_grid(sz * sy * sx, 256, 32), 256, 0, (cudaStream_t)stream>>>(volume, (int)sz, (int)sy, (int)sx, kernel_dev,
+                                                                                         (int)skz, (int)sky, (int)skx, cval, out);
   return b2v_check_launch("k_convolve_non_zero");
 }
 
@@ -388,7 +380,7 @@ namespace {
 // axis -1: the S^3 window; axis 0, 1, 2: the S x S window of every slice along that axis
 template <int S>
 void launch_median(const int16_t* in, int nz, int ny, int nx, int axis, int16_t* out, cudaStream_t s) {
-  const int g = fgrid((long long)nz * ny * nx, 128);
+  const int g = b2v_grid((long long)nz * ny * nx, 128, 32);
   if (axis < 0) k_median_i16<S, S, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
   else if (axis == 0) k_median_i16<1, S, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
   else if (axis == 1) k_median_i16<S, 1, S><<<g, 128, 0, s>>>(in, nz, ny, nx, out);
@@ -429,11 +421,11 @@ extern "C" int b2v_uniform_filter_i16(const int16_t* in, int64_t nz, int64_t ny,
   const long long n = nz * ny * nx;
   int rc;
   // SciPy filters axis 0 first (input -> output), then axes 1, 2 in place on the int16 output
-  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(in, (int)nz, (int)ny, (int)nx, 0, size, out);
+  k_uniform1d_i16<<<b2v_grid(n, 256, 32), 256, 0, s>>>(in, (int)nz, (int)ny, (int)nx, 0, size, out);
   if ((rc = b2v_check_launch("k_uniform1d_i16"))) return rc;
-  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(out, (int)nz, (int)ny, (int)nx, 1, size, tmp);
+  k_uniform1d_i16<<<b2v_grid(n, 256, 32), 256, 0, s>>>(out, (int)nz, (int)ny, (int)nx, 1, size, tmp);
   if ((rc = b2v_check_launch("k_uniform1d_i16"))) return rc;
-  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, 2, size, out);
+  k_uniform1d_i16<<<b2v_grid(n, 256, 32), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, 2, size, out);
   return b2v_check_launch("k_uniform1d_i16");
 }
 
@@ -446,9 +438,9 @@ extern "C" int b2v_uniform_filter_slices_i16(const int16_t* in, int64_t nz, int6
   const long long n = nz * ny * nx;
   const int a0 = axis == 0 ? 1 : 0, a1 = axis == 2 ? 1 : 2;   // the in-slice axes, ascending, as SciPy runs them
   int rc;
-  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(in, (int)nz, (int)ny, (int)nx, a0, size, tmp);
+  k_uniform1d_i16<<<b2v_grid(n, 256, 32), 256, 0, s>>>(in, (int)nz, (int)ny, (int)nx, a0, size, tmp);
   if ((rc = b2v_check_launch("k_uniform1d_i16"))) return rc;
-  k_uniform1d_i16<<<fgrid(n), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, a1, size, out);
+  k_uniform1d_i16<<<b2v_grid(n, 256, 32), 256, 0, s>>>(tmp, (int)nz, (int)ny, (int)nx, a1, size, out);
   return b2v_check_launch("k_uniform1d_i16");
 }
 
@@ -499,7 +491,7 @@ extern "C" int b2v_histogram_i16(const int16_t* a, int64_t n, int lo, int bins, 
     const long long g = std::max<long long>((long long)b2v_sm_count() * std::max(per_sm, 1), ceil_div64(n, 1ll << 31));
     k_histogram_i16<true><<<(int)g, 1024, smem, s>>>(a, n, lo, bins, c);
   } else {
-    k_histogram_i16<false><<<fgrid(n, 1024), 1024, 0, s>>>(a, n, lo, bins, c);
+    k_histogram_i16<false><<<b2v_grid(n, 1024, 32), 1024, 0, s>>>(a, n, lo, bins, c);
   }
   return b2v_check_launch("k_histogram_i16");
 }
@@ -512,7 +504,7 @@ extern "C" int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t
               B2V_ERR_ARG, "correlate1d: bad arguments");
   B2V_REQUIRE(nz < (1ll << 30) && ny < (1ll << 30) && nx < (1ll << 30), B2V_ERR_ARG, "correlate1d: shape too large");
   cudaStream_t s = (cudaStream_t)stream;
-  const int g = fgrid(nz * ny * nx);
+  const int g = b2v_grid(nz * ny * nx, 256, 32);
   if (in_dtype == B2V_I16 && out_dtype == B2V_I16)
     k_correlate1d<int16_t, int16_t><<<g, 256, 0, s>>>((const int16_t*)in, (int)nz, (int)ny, (int)nx, axis, weights_dev, radius, symmetry, (int16_t*)out);
   else if (in_dtype == B2V_I16 && out_dtype == B2V_F64)
@@ -528,7 +520,7 @@ extern "C" int b2v_correlate1d(const void* in, int in_dtype, int64_t nz, int64_t
 extern "C" int b2v_sharpen_i16(const int16_t* img, const double* blurred, int64_t n, double value, double lo, double hi,
                                int16_t* out, void* stream) {
   B2V_REQUIRE(img && blurred && out && n > 0, B2V_ERR_ARG, "sharpen: bad arguments");
-  k_sharpen<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5, ClipWhole{lo, hi}, out);
+  k_sharpen<<<b2v_grid(n, 256, 32), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5, ClipWhole{lo, hi}, out);
   return b2v_check_launch("k_sharpen");
 }
 
@@ -537,22 +529,22 @@ extern "C" int b2v_sharpen_slices_i16(const int16_t* img, const double* blurred,
   B2V_REQUIRE(img && blurred && minmax_dev && out && nz > 0 && ny > 0 && nx > 0 && valid_slice_axis(axis), B2V_ERR_ARG,
               "sharpen_slices: bad arguments");
   const long long n = nz * ny * nx;
-  k_sharpen<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5,
-                                                        ClipPerSlice{minmax_dev, slice_of(ny, nx, axis, nz)}, out);
+  k_sharpen<<<b2v_grid(n, 256, 32), 256, 0, (cudaStream_t)stream>>>(img, blurred, n, value * 0.5,
+                                                                    ClipPerSlice{minmax_dev, slice_of(ny, nx, axis, nz)}, out);
   return b2v_check_launch("k_sharpen");
 }
 
 extern "C" int b2v_sobel_magnitude(double* sx_inout, const double* sy, const double* sz, int64_t n, void* stream) {
   B2V_REQUIRE(sx_inout && sy && n > 0, B2V_ERR_ARG, "sobel_magnitude: bad arguments");
-  k_sobel_magnitude<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(sx_inout, sy, sz, n);
+  k_sobel_magnitude<<<b2v_grid(n, 256, 32), 256, 0, (cudaStream_t)stream>>>(sx_inout, sy, sz, n);
   return b2v_check_launch("k_sobel_magnitude");
 }
 
 extern "C" int b2v_rescale_cast_i16(const double* m, int64_t n, int rescale, double mag_min, double mag_range, double span,
                                     double min_val, int16_t* out, void* stream) {
   B2V_REQUIRE(m && out && n > 0, B2V_ERR_ARG, "rescale_cast: bad arguments");
-  k_rescale_cast<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(m, n, RescaleWhole{{rescale, mag_min, mag_range, span, min_val}},
-                                                             out);
+  k_rescale_cast<<<b2v_grid(n, 256, 32), 256, 0, (cudaStream_t)stream>>>(m, n, RescaleWhole{{rescale, mag_min, mag_range, span, min_val}},
+                                                                         out);
   return b2v_check_launch("k_rescale_cast");
 }
 
@@ -562,7 +554,7 @@ extern "C" int b2v_rescale_cast_slices_i16(const double* m, int64_t nz, int64_t 
   B2V_REQUIRE(m && mag_minmax_dev && img_minmax_dev && out && nz > 0 && ny > 0 && nx > 0 && valid_slice_axis(axis),
               B2V_ERR_ARG, "rescale_cast_slices: bad arguments");
   const long long n = nz * ny * nx;
-  k_rescale_cast<<<fgrid(n), 256, 0, (cudaStream_t)stream>>>(
+  k_rescale_cast<<<b2v_grid(n, 256, 32), 256, 0, (cudaStream_t)stream>>>(
       m, n, RescalePerSlice{mag_minmax_dev, img_minmax_dev, slice_of(ny, nx, axis, nz)}, out);
   return b2v_check_launch("k_rescale_cast");
 }

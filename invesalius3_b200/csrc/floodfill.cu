@@ -1097,14 +1097,6 @@ int check_seeds(const int64_t* seeds_host, int64_t nseeds, int64_t dz, int64_t d
   return B2V_OK;
 }
 
-int grid_for(int64_t items, int per_block) {
-  int64_t blocks = ceil_div64(items, per_block);
-  int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 // rounds until no tile is active. Synchronises the stream (reads one flag per batch).
 int run_rounds(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_t s, int r0, int* rounds_out) {
   const int ntiles = b.ntz * b.nty * b.ntw;
@@ -1241,14 +1233,15 @@ int flood(T* data, uint8_t* out, int64_t dz, int64_t dy, int64_t dx, const int64
                ((uintptr_t)out & 7u) == 0;
     if (vec) {
       if (dx % 32 == 0)
-        k_ff_build_i16_vec<MODE, true><<<grid_for(nwords * 4, 1024), 256, 0, s>>>((const int16_t*)data, out, b, (int)t0,
-                                                                                 (int)t1, fill_o, w.fg, w.reach);
+        k_ff_build_i16_vec<MODE, true><<<b2v_grid(nwords * 4, 1024, 16), 256, 0, s>>>((const int16_t*)data, out, b,
+                                                                                      (int)t0, (int)t1, fill_o, w.fg,
+                                                                                      w.reach);
       else
-        k_ff_build_i16_vec<MODE, false><<<grid_for(nwords * 4, 1024), 256, 0, s>>>((const int16_t*)data, out, b,
-                                                                                  (int)t0, (int)t1, fill_o, w.fg,
-                                                                                  w.reach);
+        k_ff_build_i16_vec<MODE, false><<<b2v_grid(nwords * 4, 1024, 16), 256, 0, s>>>((const int16_t*)data, out, b,
+                                                                                       (int)t0, (int)t1, fill_o, w.fg,
+                                                                                       w.reach);
     } else {
-      k_ff_build<T, MODE><<<grid_for(nwords, 8), 256, 0, s>>>(data, out, b, t0, t1, fill_t, fill_o, w.fg, w.reach);
+      k_ff_build<T, MODE><<<b2v_grid(nwords, 8, 16), 256, 0, s>>>(data, out, b, t0, t1, fill_t, fill_o, w.fg, w.reach);
     }
     if ((rc = b2v_check_launch("k_ff_build"))) return rc;
     if (nseeds) {
@@ -1272,9 +1265,9 @@ int flood(T* data, uint8_t* out, int64_t dz, int64_t dy, int64_t dx, const int64
   }
   if (stages & STAGE_FINISH) {
     if (MODE == MODE_INPLACE)
-      k_ff_write<T><<<grid_for(nwords, 8), 256, 0, s>>>(w.reach, b, (T)fill_t, data);
+      k_ff_write<T><<<b2v_grid(nwords, 8, 16), 256, 0, s>>>(w.reach, b, (T)fill_t, data);
     else
-      k_ff_write<uint8_t><<<grid_for(nwords, 8), 256, 0, s>>>(w.reach, b, fill_o, out);
+      k_ff_write<uint8_t><<<b2v_grid(nwords, 8, 16), 256, 0, s>>>(w.reach, b, fill_o, out);
     if ((rc = b2v_check_launch("k_ff_write"))) return rc;
   }
   if (verdict_due) {
@@ -1516,7 +1509,7 @@ extern "C" int b2v_fill_holes_staged(int stages, uint8_t* mask, const uint32_t* 
   if (stages & 1) {
     B2V_CUDA(cudaMemsetAsync(workspace, 0, (size_t)(256 + nbins * 4), s));
     if (n > 0) {
-      k_fh_hist<<<grid_for(n, 256 * 8), 256, 0, s>>>(labels, n, nlabels, sizes, ctrl + 1);
+      k_fh_hist<<<b2v_grid(n, 256 * 8, 16), 256, 0, s>>>(labels, n, nlabels, sizes, ctrl + 1);
       if ((rc = b2v_check_launch("k_fh_hist"))) return rc;
     }
   }
@@ -1524,7 +1517,7 @@ extern "C" int b2v_fill_holes_staged(int stages, uint8_t* mask, const uint32_t* 
     k_fh_any<<<(unsigned)ceil_div64(nbins, 256), 256, 0, s>>>(sizes, nbins, max_size, ctrl);
     if ((rc = b2v_check_launch("k_fh_any"))) return rc;
     if (n > 0) {
-      k_fh_apply<<<grid_for(n, 256), 256, 0, s>>>(labels, n, sizes, nlabels, max_size, ctrl, mask);
+      k_fh_apply<<<b2v_grid(n, 256, 16), 256, 0, s>>>(labels, n, sizes, nlabels, max_size, ctrl, mask);
       if ((rc = b2v_check_launch("k_fh_apply"))) return rc;
     }
     int host[2] = {0, 0};

@@ -205,19 +205,11 @@ __global__ void __launch_bounds__(256) k_count_gather(const T* __restrict__ img,
   }
 }
 
-int lgrid(long long n) {
-  long long blocks = ceil_div64(n, 256 * 4);
-  long long cap = (long long)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 }  // namespace
 
 extern "C" int64_t b2v_label_workspace_bytes(int64_t n) {
   if (n <= 0) return 0;
-  return ((n * 4 + 255) & ~(int64_t)255) + ((ceil_div64(n, kScanBlock) + 1) * 4 + 255 & ~(int64_t)255) + 256;
+  return align256(n * 4) + align256((ceil_div64(n, kScanBlock) + 1) * 4) + 256;
 }
 
 extern "C" int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t nx, const uint8_t* strct_host, int64_t odz,
@@ -239,12 +231,12 @@ extern "C" int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t n
   cudaStream_t s = (cudaStream_t)stream;
   LDims d = {(int)nz, (int)ny, (int)nx, nz * ny * nx};
   int* parent = (int*)workspace;
-  uint32_t* bsum = (uint32_t*)((char*)workspace + ((d.n * 4 + 255) & ~(long long)255));
+  uint32_t* bsum = (uint32_t*)((char*)workspace + align256(d.n * 4));
   const long long nb = ceil_div64(d.n, kScanBlock);
   int rc;
-  k_label_init<<<lgrid(d.n), 256, 0, s>>>(input, d, parent);
+  k_label_init<<<b2v_grid(d.n, 256 * 4, 16), 256, 0, s>>>(input, d, parent);
   if ((rc = b2v_check_launch("k_label_init"))) return rc;
-  k_label_merge<<<lgrid(d.n), 256, 0, s>>>(input, d, sb, parent);
+  k_label_merge<<<b2v_grid(d.n, 256 * 4, 16), 256, 0, s>>>(input, d, sb, parent);
   if ((rc = b2v_check_launch("k_label_merge"))) return rc;
   k_label_flatten_count<<<(unsigned)nb, 256, 0, s>>>(parent, d, labels, bsum);
   if ((rc = b2v_check_launch("k_label_flatten_count"))) return rc;
@@ -252,7 +244,7 @@ extern "C" int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t n
   if ((rc = b2v_check_launch("k_label_scan_bsums"))) return rc;
   k_label_number_roots<<<(unsigned)nb, 256, 0, s>>>(parent, d, bsum, labels);
   if ((rc = b2v_check_launch("k_label_number_roots"))) return rc;
-  k_label_assign<<<lgrid(d.n), 256, 0, s>>>(parent, d, labels);
+  k_label_assign<<<b2v_grid(d.n, 256 * 4, 16), 256, 0, s>>>(parent, d, labels);
   if ((rc = b2v_check_launch("k_label_assign"))) return rc;
   uint32_t total = 0;
   B2V_CUDA(cudaMemcpyAsync(&total, bsum + nb, 4, cudaMemcpyDeviceToHost, s));
@@ -271,13 +263,13 @@ extern "C" int b2v_count_regions(const void* image, int dtype, int64_t n, uint32
   B2V_CUDA(cudaMemsetAsync(workspace, 0, 256 + (size_t)nbins * 4, s));
   int rc;
   if (dtype == B2V_I16) {
-    k_count_hist<int16_t><<<lgrid(n), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, status);
+    k_count_hist<int16_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, status);
     if ((rc = b2v_check_launch("k_count_hist"))) return rc;
-    k_count_gather<int16_t><<<lgrid(n), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, out);
+    k_count_gather<int16_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, out);
   } else if (dtype == B2V_U8) {
-    k_count_hist<uint8_t><<<lgrid(n), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, status);
+    k_count_hist<uint8_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, status);
     if ((rc = b2v_check_launch("k_count_hist"))) return rc;
-    k_count_gather<uint8_t><<<lgrid(n), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, out);
+    k_count_gather<uint8_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, out);
   } else {
     B2V_REQUIRE(false, B2V_ERR_ARG, "count_regions: image must be int16 or uint8");
   }

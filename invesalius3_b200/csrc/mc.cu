@@ -68,15 +68,14 @@ struct McWs {
 
 McWs carve(void* base, const McGeom& g) {
   McWs w;
-  auto align = [](int64_t v) { return (v + 255) & ~(int64_t)255; };
   char* p = (char*)base;
   int64_t off = 0;
   const int64_t ntiles = ceil_div64(g.nwords, kTileWords);
-  w.bits = (uint32_t*)(p + off); off += align(g.nwords * 4 + 64);
-  w.vrec = (uint4*)(p + off); off += align(ntiles * kTileWords * 16);
-  w.tcnt = (uint4*)(p + off); off += align(ntiles * 16);
-  w.toff = (uint4*)(p + off); off += align(ntiles * 16);
-  w.plane0 = (uint4*)(p + off); off += align(g.ny * g.wx * 16);
+  w.bits = (uint32_t*)(p + off); off += align256(g.nwords * 4 + 64);
+  w.vrec = (uint4*)(p + off); off += align256(ntiles * kTileWords * 16);
+  w.tcnt = (uint4*)(p + off); off += align256(ntiles * 16);
+  w.toff = (uint4*)(p + off); off += align256(ntiles * 16);
+  w.plane0 = (uint4*)(p + off); off += align256(g.ny * g.wx * 16);
   const int64_t ctl0 = off;
   w.totals = (unsigned long long*)(p + off); off += 256;
   w.ticket = (unsigned int*)(p + off); off += 256;
@@ -709,14 +708,6 @@ __global__ void __launch_bounds__(kTileThreads) k_mc_emit_tris(McGeom g, const u
   }
 }
 
-int grid_for(int64_t items, int per_block) {
-  int64_t blocks = ceil_div64(items, per_block);
-  int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 __global__ void k_mc_pack_tables() {
   signed char e[16];
   for (int k = 0; k < 15; ++k) e[k] = B2V_MC_TRI[threadIdx.x][k];
@@ -770,17 +761,17 @@ static int mc_count_impl(const void* vol, int dtype, int64_t nz, int64_t ny, int
     int thr = int_threshold(iso, 0, 255);
     if (nx % 16 == 0 && b2v_aligned16(vol))
       if (nx % 32 == 0)
-        k_mc_bits_u8_vec<true><<<grid_for(g.nwords * 2, 1024), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
+        k_mc_bits_u8_vec<true><<<b2v_grid(g.nwords * 2, 1024, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
       else
-        k_mc_bits_u8_vec<false><<<grid_for(g.nwords * 2, 1024), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
+        k_mc_bits_u8_vec<false><<<b2v_grid(g.nwords * 2, 1024, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
     else
-      k_mc_bits<uint8_t><<<grid_for(g.nwords, 8), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
+      k_mc_bits<uint8_t><<<b2v_grid(g.nwords, 8, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
   } else {
     int thr = int_threshold(iso, -32768, 32767);
     if (nx % 8 == 0 && b2v_aligned16(vol))
-      k_mc_bits_i16_vec<<<grid_for(g.nwords * 4, 256), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
+      k_mc_bits_i16_vec<<<b2v_grid(g.nwords * 4, 256, 16), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
     else
-      k_mc_bits<int16_t><<<grid_for(g.nwords, 8), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
+      k_mc_bits<int16_t><<<b2v_grid(g.nwords, 8, 16), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
   }
   if ((rc = b2v_check_launch("k_mc_bits"))) return rc;
   const int ntiles = (int)ceil_div64(g.nwords, kTileWords);

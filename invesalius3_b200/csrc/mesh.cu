@@ -21,14 +21,6 @@
 
 namespace {
 
-int mgrid(long long n) {
-  long long blocks = ceil_div64(n, 256);
-  long long cap = (long long)b2v_sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 struct MeshWs {
   long long* first;     // [V] start of the vertex's entries in `order` (-1: none)
   long long* last;      // [V]
@@ -47,21 +39,20 @@ struct MeshWs {
 
 MeshWs carve(void* base, long long nv, long long nf) {
   MeshWs w;
-  auto al = [](long long v) { return (v + 255) & ~255ll; };
   char* p = (char*)base;
   long long off = 0;
-  w.first = (long long*)(p + off); off += al(nv * 8);
-  w.last = (long long*)(p + off); off += al(nv * 8);
-  w.deg = (uint32_t*)(p + off); off += al((nv + 1) * 4);
-  w.adj = (uint32_t*)(p + off); off += al(6 * nf * 4 + 4);
-  w.bsum = (uint32_t*)(p + off); off += al((ceil_div64(nv + 1, 2048) + 2) * 4);
-  w.dist = (unsigned long long*)(p + off); off += al(nv * 8);
-  w.seed = (int*)(p + off); off += al(nv * 4);
-  w.frontier[0] = (int*)(p + off); off += al(6 * nf * 4 + nv * 4 + 4);
-  w.frontier[1] = (int*)(p + off); off += al(6 * nf * 4 + nv * 4 + 4);
+  w.first = (long long*)(p + off); off += align256(nv * 8);
+  w.last = (long long*)(p + off); off += align256(nv * 8);
+  w.deg = (uint32_t*)(p + off); off += align256((nv + 1) * 4);
+  w.adj = (uint32_t*)(p + off); off += align256(6 * nf * 4 + 4);
+  w.bsum = (uint32_t*)(p + off); off += align256((ceil_div64(nv + 1, 2048) + 2) * 4);
+  w.dist = (unsigned long long*)(p + off); off += align256(nv * 8);
+  w.seed = (int*)(p + off); off += align256(nv * 4);
+  w.frontier[0] = (int*)(p + off); off += align256(6 * nf * 4 + nv * 4 + 4);
+  w.frontier[1] = (int*)(p + off); off += align256(6 * nf * 4 + nv * 4 + 4);
   w.fcount = (int*)(p + off); off += 256;
-  w.w = (double*)(p + off); off += al(nv * 8);
-  w.d = (double*)(p + off); off += al(nv * 24);
+  w.w = (double*)(p + off); off += align256(nv * 8);
+  w.d = (double*)(p + off); off += align256(nv * 24);
   w.status = (int*)(p + off); off += 256;
   w.bytes = off;
   return w;
@@ -317,14 +308,15 @@ extern "C" int b2v_ca_smoothing(float* vertices, int64_t nverts, const int64_t* 
   cudaStream_t s = (cudaStream_t)stream;
   MeshWs w = carve(workspace, nverts, nfaces);
   unsigned long long* dist_before = (unsigned long long*)((char*)workspace + w.bytes);
-  int* seed_new = (int*)((char*)dist_before + ((nverts * 8 + 255) & ~255ll));
+  int* seed_new = (int*)((char*)dist_before + align256(nverts * 8));
   const long long ne = 4 * nfaces, nv = nverts;
   int rc;
   B2V_CUDA(cudaMemsetAsync(w.status, 0, 4, s));
   B2V_CUDA(cudaMemsetAsync(w.fcount, 0, 16, s));
   k_fill_i64<<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(w.first, nv, -1);
   k_fill_int<<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(seed_new, nv, 0x7fffffff);
-  k_mesh_segments<<<mgrid(ne), 256, 0, s>>>((const long long*)faces4, (const long long*)order, ne, nv, w.first, w.last, w.status);
+  k_mesh_segments<<<b2v_grid(ne, 256, 32), 256, 0, s>>>((const long long*)faces4, (const long long*)order, ne, nv,
+                                                        w.first, w.last, w.status);
   if ((rc = b2v_check_launch("k_mesh_segments"))) return rc;
   int st = 0;
   B2V_CUDA(cudaMemcpyAsync(&st, w.status, 4, cudaMemcpyDeviceToHost, s));

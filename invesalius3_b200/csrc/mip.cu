@@ -325,13 +325,11 @@ int run_keepx(const T* img, const KeepX& g, void* out, void* ws, cudaStream_t st
 
 template <typename T, int KIND>
 int run_alongx(const T* img, int64_t nrows, int64_t nx, void* out, cudaStream_t st) {
-  int64_t blocks = ceil_div64(nrows, 8);
-  int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
+  const int blocks = b2v_grid(nrows, 8, 16);
   if (sizeof(T) == 2 && b2v_aligned16(img) && nx % 8 == 0)
-    k_alongx_i16_vec<KIND><<<(unsigned)blocks, 256, 0, st>>>((const int16_t*)img, nrows, nx, out);
+    k_alongx_i16_vec<KIND><<<blocks, 256, 0, st>>>((const int16_t*)img, nrows, nx, out);
   else
-    k_alongx_scalar<T, KIND><<<(unsigned)blocks, 256, 0, st>>>(img, nrows, nx, out);
+    k_alongx_scalar<T, KIND><<<blocks, 256, 0, st>>>(img, nrows, nx, out);
   return b2v_check_launch("k_alongx");
 }
 
@@ -390,10 +388,7 @@ __global__ void __launch_bounds__(256) k_mip_f64_alongx(const double* __restrict
 int run_mip_f64(const double* img, int64_t dz, int64_t dy, int64_t dx, int axis, int kind, double* out, cudaStream_t st) {
   B2V_REQUIRE(kind == KMAX || kind == KMIN, B2V_ERR_ARG, "mip: MeanIP of a float64 volume is not built (NumPy sums pairwise)");
   if (axis == 2) {
-    int64_t blocks = ceil_div64(dz * dy, 8);
-    int64_t cap = (int64_t)b2v_sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    k_mip_f64_alongx<<<(unsigned)blocks, 256, 0, st>>>(img, dz * dy, dx, kind == KMAX, out);
+    k_mip_f64_alongx<<<b2v_grid(dz * dy, 8, 16), 256, 0, st>>>(img, dz * dy, dx, kind == KMAX, out);
     return b2v_check_launch("k_mip_f64_alongx");
   }
   KeepX g = keepx_geom(dz, dy, dx, axis);

@@ -607,7 +607,6 @@ extern "C" int b2v_fcm_volume(const void* img, int dtype, int64_t dz, int64_t dy
 }
 
 static int64_t dtype_bytes(int dtype) { return dtype == B2V_I16 ? 2 : (dtype == B2V_U8 ? 1 : 8); }
-static int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
 
 // workspace of b2v_fast_countour_mip: [projection workspace | contour volume | MaxIP workspace]
 extern "C" int64_t b2v_fcm_workspace_bytes(int dtype, int64_t dz, int64_t dy, int64_t dx, int axis, int tmip) {

@@ -309,8 +309,6 @@ double pw_combine(int64_t n, const double* part, size_t* idx) {
 
 int64_t max_subtrees(int64_t n) { return n / (kSub / 4) + 2; }   // every subtree of a split holds > kSub/2 - 8
 
-int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 struct MomentsLayout { int64_t counts, offsets, vals, subs, part, total; };
 MomentsLayout moments_layout(int64_t n) {
   const int64_t nt = ceil_div64(n, kTile), ms = max_subtrees(n);
@@ -324,17 +322,10 @@ MomentsLayout moments_layout(int64_t n) {
   return L;
 }
 
-int grid_for(int64_t n) {
-  int64_t blocks = ceil_div64(n, 256 * 4);
-  const int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  return (int)(blocks < 1 ? 1 : blocks);
-}
-
 template <typename T>
 int lut_launch(const void* img, int64_t n, double window, double level, void* out, cudaStream_t s) {
   const double c = level - 0.5, lo = level - 0.5 - (window - 1.0) / 2.0, hi = level - 0.5 + (window - 1.0) / 2.0;
-  k_lut255<T><<<grid_for(n), 256, 0, s>>>((const T*)img, n, lo, hi, c, window - 1.0, (T*)out);
+  k_lut255<T><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const T*)img, n, lo, hi, c, window - 1.0, (T*)out);
   return b2v_check_launch("k_lut255");
 }
 

@@ -167,13 +167,9 @@ extern "C" int b2v_threshold_i16(const int16_t* img, int64_t n, int32_t lo, int3
     done = ngroups * 16;
   }
   if (done < n) {
-    int64_t rem = n - done;
-    int64_t blocks = ceil_div64(rem, 256);
-    int64_t cap = (int64_t)b2v_sm_count() * 16;
-    if (blocks > cap) blocks = cap;
     // an empty range is expressed to the scalar kernel as lo > hi
-    k_threshold_scalar<<<(unsigned)blocks, 256, 0, s>>>(img, mask, done, n, r.none ? 1 : r.lo, r.none ? 0 : r.hi,
-                                                        preserve_markers);
+    k_threshold_scalar<<<b2v_grid(n - done, 256, 16), 256, 0, s>>>(img, mask, done, n, r.none ? 1 : r.lo,
+                                                                   r.none ? 0 : r.hi, preserve_markers);
     if ((rc = b2v_check_launch("k_threshold_scalar"))) return rc;
   }
   return B2V_OK;
@@ -186,12 +182,8 @@ extern "C" int b2v_threshold_i16_masklayout(const int16_t* img, int64_t dz, int6
   B2V_REQUIRE(dz > 0 && dy > 0 && dx > 0, B2V_ERR_ARG, "threshold_masklayout: empty volume");
   cudaStream_t s = (cudaStream_t)stream;
   Range r = clamp_range(lo, hi);
-  int64_t nrows = dz * dy;
-  int64_t blocks = ceil_div64(nrows, 8);
-  int64_t cap = (int64_t)b2v_sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  k_threshold_masklayout<<<(unsigned)blocks, 256, 0, s>>>(img, mask_padded, dz, dy, dx, r.none ? 1 : r.lo,
-                                                          r.none ? 0 : r.hi, preserve_markers, only_dirty);
+  k_threshold_masklayout<<<b2v_grid(dz * dy, 8, 32), 256, 0, s>>>(img, mask_padded, dz, dy, dx, r.none ? 1 : r.lo,
+                                                                  r.none ? 0 : r.hi, preserve_markers, only_dirty);
   int rc;
   if ((rc = b2v_check_launch("k_threshold_masklayout"))) return rc;
   k_set_axial_flags<<<(unsigned)ceil_div64(dz, 256), 256, 0, s>>>(mask_padded, dz, (dy + 1) * (dx + 1));

@@ -150,13 +150,9 @@ __global__ void __launch_bounds__(256) k_view_transform(const T* __restrict__ vo
 template <typename T>
 int run_view_transform(const void* vol, VDims d, const double* sp, const Mat4& M, long long n, int orientation,
                        int minterpol, double cval, void* out, VDims od, int* status, cudaStream_t s) {
-  long long total = od.dz * od.dy * od.dx;
-  long long blocks = ceil_div64(total, 256);
-  long long cap = (long long)b2v_sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  k_view_transform<T><<<(unsigned)blocks, 256, 0, s>>>((const T*)vol, d, sp[0], sp[1], sp[2], M, n, orientation, minterpol,
-                                                      (T)cval, (T*)out, od, status);
+  k_view_transform<T><<<b2v_grid(od.dz * od.dy * od.dx, 256, 32), 256, 0, s>>>((const T*)vol, d, sp[0], sp[1], sp[2], M,
+                                                                               n, orientation, minterpol, (T)cval,
+                                                                               (T*)out, od, status);
   return b2v_check_launch("k_view_transform");
 }
 

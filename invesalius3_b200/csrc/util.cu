@@ -186,13 +186,8 @@ __global__ void __launch_bounds__(256) k_minmax_final(const float2* __restrict__
   }
 }
 
-static int minmax_blocks(int64_t n) {
-  int64_t want = ceil_div64(n, 256 * 16);
-  int64_t cap = (int64_t)b2v_sm_count() * 8;
-  if (want > cap) want = cap;
-  if (want < 1) want = 1;
-  return (int)want;
-}
+// one partial per block: the workspace size and the launch must agree
+static int minmax_blocks(int64_t n) { return b2v_grid(n, 256 * 16, 8); }
 
 extern "C" int64_t b2v_minmax_workspace_bytes(int64_t n) { return (int64_t)minmax_blocks(n) * sizeof(float2); }
 

@@ -53,7 +53,7 @@ constexpr int kBlock = 256;
 constexpr int kCamDoubles = B2V_VIS_CAMERA_DOUBLES;
 constexpr unsigned long long kDepthOne = 0x3FF0000000000000ull;   // bits of 1.0
 
-enum : uint32_t { ST_BAD_FACE = 1u, ST_NONFINITE = 2u };
+enum : uint32_t { ST_NONFINITE = 2u };   // a status bit beside ST_BAD_FACE (1)
 
 struct P3 { double x, y, z; };
 
@@ -190,8 +190,6 @@ struct VisWs {
   size_t bytes;
 };
 
-inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
-
 uint64_t hash_slots(int64_t nv) {
   uint64_t h = 1024;
   while (h < 2 * (uint64_t)nv) h <<= 1;
@@ -202,7 +200,7 @@ VisWs carve(void* base, int64_t nv, int64_t nt, int nviews) {
   VisWs w;
   char* p = (char*)base;
   size_t o = 0;
-  auto take = [&](size_t n) { char* r = p + o; o += al(n); return r; };
+  auto take = [&](size_t n) { char* r = p + o; o += align256(n); return r; };
   const uint64_t H = hash_slots(nv);
   w.hmask = H - 1;
   w.nb = ceil_div64(nt, kBlock);
@@ -235,34 +233,6 @@ __host__ __forceinline__ float key_to_float(uint32_t k) {
   memcpy(&f, &u, 4);
   return f;
 }
-
-struct Faces {
-  const void* p;
-  int64_t nt;
-  int cols;    // 3, or 4 with a leading 3
-  int i64;
-  int64_t nv;
-};
-
-// the three vertex ids of face t; false when the face is malformed (an index outside [0, nv) or a leading
-// entry other than 3 in the [T, 4] form)
-__device__ __forceinline__ bool load_face(const Faces& F, int64_t t, int64_t v[3]) {
-  const int64_t base = t * F.cols;
-  const int off = F.cols == 4 ? 1 : 0;
-  if (F.i64) {
-    const int64_t* f = (const int64_t*)F.p + base;
-    if (off && f[0] != 3) return false;
-    v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
-  } else {
-    const int32_t* f = (const int32_t*)F.p + base;
-    if (off && f[0] != 3) return false;
-    v[0] = f[off]; v[1] = f[off + 1]; v[2] = f[off + 2];
-  }
-  return v[0] >= 0 && v[0] < F.nv && v[1] >= 0 && v[1] < F.nv && v[2] >= 0 && v[2] < F.nv;
-}
-
-__device__ __forceinline__ int64_t gtid() { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; }
-__device__ __forceinline__ int64_t gstride() { return (int64_t)gridDim.x * blockDim.x; }
 
 // ---- bounds -----------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kBlock) k_vis_bounds(const float* __restrict__ v, int64_t nv, uint32_t* misc) {
@@ -502,33 +472,6 @@ __device__ __forceinline__ FaceFlags face_flags(const Faces& F, int64_t t, const
   return o;
 }
 
-// block-wide exclusive scan (kBlock threads); returns the prefix and the block total
-template <typename T>
-__device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  T inc = x;
-  for (int o = 1; o < 32; o <<= 1) {
-    const T y = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += y;
-  }
-  if (lane == 31) s_w[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    const int nw = blockDim.x >> 5;
-    T w = lane < nw ? s_w[lane] : 0;
-    for (int o = 1; o < 32; o <<= 1) {
-      const T y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    if (lane < nw) s_w[lane] = w;
-  }
-  __syncthreads();
-  const T base = wid ? s_w[wid - 1] : 0;
-  *total = s_w[(blockDim.x >> 5) - 1];
-  __syncthreads();
-  return base + inc - x;
-}
-
 __global__ void __launch_bounds__(kBlock) k_vis_block_counts(Faces F, const uint8_t* __restrict__ vis, uint8_t flip,
                                                              const uint32_t* __restrict__ rep,
                                                              const unsigned long long* __restrict__ first,
@@ -599,13 +542,6 @@ __global__ void __launch_bounds__(kBlock) k_vis_emit_faces(Faces F, const uint8_
   const uint64_t id = boff[blockIdx.x] + block_exscan<uint32_t>((uint32_t)f.emit, s_w, &tot);
   if (!f.emit) return;
   for (int c = 0; c < 3; ++c) out[3 * id + c] = newid[f.r[c]];
-}
-
-unsigned grid_for(int64_t n, int per_sm) {
-  int64_t b = ceil_div64(n, kBlock);
-  const int64_t cap = (int64_t)b2v_sm_count() * per_sm;
-  if (b > cap) b = cap;
-  return (unsigned)(b < 1 ? 1 : b);
 }
 
 int check_mesh(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
@@ -683,7 +619,7 @@ extern "C" int b2v_visibility_bounds(const float* verts, int64_t nv, void* works
   uint32_t init[8] = {0xffffffffu, 0, 0xffffffffu, 0, 0xffffffffu, 0, 0, 0};
   uint32_t* misc = (uint32_t*)workspace;
   B2V_CUDA(cudaMemcpyAsync(misc, init, sizeof(init), cudaMemcpyHostToDevice, s));
-  k_vis_bounds<<<grid_for(nv, 8), kBlock, 0, s>>>(verts, nv, misc);
+  k_vis_bounds<<<b2v_grid(nv, kBlock, 8), kBlock, 0, s>>>(verts, nv, misc);
   if (int rc = b2v_check_launch("k_vis_bounds")) return rc;
   uint32_t got[8];
   B2V_CUDA(cudaMemcpyAsync(got, misc, sizeof(got), cudaMemcpyDeviceToHost, s));
@@ -712,23 +648,24 @@ extern "C" int b2v_visibility_count(const float* verts, int64_t nv, const void* 
   B2V_CUDA(cudaMemsetAsync(w.slots, 0xff, (w.hmask + 1) * 4, s));
   B2V_CUDA(cudaMemsetAsync(w.first, 0xff, (w.hmask + 1) * 8, s));
 
-  k_vis_fill_u64<<<grid_for((int64_t)nviews * kPix, 8), kBlock, 0, s>>>(w.zbuf, (int64_t)nviews * kPix, kDepthOne);
+  k_vis_fill_u64<<<b2v_grid((int64_t)nviews * kPix, kBlock, 8), kBlock, 0, s>>>(w.zbuf, (int64_t)nviews * kPix,
+                                                                                kDepthOne);
   if (int rc = b2v_check_launch("k_vis_fill_u64")) return rc;
-  k_vis_project<<<grid_for((int64_t)nviews * nv, 16), kBlock, 0, s>>>(verts, nv, nviews, w.cams, w.proj);
+  k_vis_project<<<b2v_grid((int64_t)nviews * nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, nviews, w.cams, w.proj);
   if (int rc = b2v_check_launch("k_vis_project")) return rc;
-  k_vis_merge_insert<<<grid_for(nv, 16), kBlock, 0, s>>>(verts, nv, w.hmask, w.slots, w.rep);
+  k_vis_merge_insert<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, w.hmask, w.slots, w.rep);
   if (int rc = b2v_check_launch("k_vis_merge_insert")) return rc;
   if (nt > 0) {
-    k_vis_raster<<<grid_for((int64_t)nviews * nt, 16), kBlock, 0, s>>>(F, nviews, w.proj, w.zbuf, w.queue, w.qcount,
-                                                                      w.misc);
+    k_vis_raster<<<b2v_grid((int64_t)nviews * nt, kBlock, 16), kBlock, 0, s>>>(F, nviews, w.proj, w.zbuf, w.queue,
+                                                                               w.qcount, w.misc);
     if (int rc = b2v_check_launch("k_vis_raster")) return rc;
     k_vis_raster_big<<<(unsigned)b2v_sm_count() * 4, kBlock, 0, s>>>(F, w.proj, w.zbuf, w.queue, w.qcount);
     if (int rc = b2v_check_launch("k_vis_raster_big")) return rc;
   }
-  k_vis_points<<<grid_for(nv, 16), kBlock, 0, s>>>(nv, nviews, w.proj, w.zbuf, w.vis);
+  k_vis_points<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(nv, nviews, w.proj, w.zbuf, w.vis);
   if (int rc = b2v_check_launch("k_vis_points")) return rc;
   if (nt > 0) {
-    k_vis_first_use<<<grid_for(nt, 16), kBlock, 0, s>>>(F, w.vis, flip, w.rep, w.first);
+    k_vis_first_use<<<b2v_grid(nt, kBlock, 16), kBlock, 0, s>>>(F, w.vis, flip, w.rep, w.first);
     if (int rc = b2v_check_launch("k_vis_first_use")) return rc;
     B2V_REQUIRE(w.nb <= 0x7fffffffLL, B2V_ERR_ARG, "visibility_count: too many faces");
     k_vis_block_counts<<<(unsigned)w.nb, kBlock, 0, s>>>(F, w.vis, flip, w.rep, w.first, w.bcount, w.nb);

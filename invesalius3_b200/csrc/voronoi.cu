@@ -234,8 +234,6 @@ struct Layout {
   int64_t own_b, dist_b, site_f, count, sum, max_bits, centroid, total;
 };
 
-int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 Layout layout(int64_t nvox, int64_t n) {
   Layout L;
   L.own_b = 0;
@@ -348,9 +346,6 @@ extern "C" int b2v_image_normalize_f32_i16(const float* in, int64_t n, float imi
   B2V_REQUIRE(n >= 0, B2V_ERR_ARG, "image_normalize: negative size");
   if (n == 0) return B2V_OK;
   B2V_REQUIRE(in && out, B2V_ERR_ARG, "image_normalize: null pointer");
-  int64_t blocks = ceil_div64(n, 256);
-  const int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  k_image_normalize<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(in, n, imin, imax, span, min_f, fill, out);
+  k_image_normalize<<<b2v_grid(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(in, n, imin, imax, span, min_f, fill, out);
   return b2v_check_launch("k_image_normalize");
 }

@@ -172,16 +172,15 @@ struct WsWs {
 };
 WsWs carve(void* base, const Grid& g) {
   WsWs w;
-  auto align = [](int64_t v) { return (v + 255) & ~(int64_t)255; };
   int64_t n = g.nz * g.ny * g.nx, nt = (int64_t)g.ntz * g.nty * g.ntx;
   char* p = (char*)base;
   int64_t off = 0;
-  w.key = (unsigned long long*)(p + off); off += align(n * 8);
-  w.cost = (uint32_t*)(p + off); off += align(n * 4);
-  w.lset = (uint16_t*)(p + off); off += align(n * 2);
-  w.active[0] = (uint8_t*)(p + off); off += align(nt);
-  w.active[1] = (uint8_t*)(p + off); off += align(nt);
-  w.flags = (int*)(p + off); off += align((int64_t)(kMaxRounds + 2) * 4);
+  w.key = (unsigned long long*)(p + off); off += align256(n * 8);
+  w.cost = (uint32_t*)(p + off); off += align256(n * 4);
+  w.lset = (uint16_t*)(p + off); off += align256(n * 2);
+  w.active[0] = (uint8_t*)(p + off); off += align256(nt);
+  w.active[1] = (uint8_t*)(p + off); off += align256(nt);
+  w.flags = (int*)(p + off); off += align256((int64_t)(kMaxRounds + 2) * 4);
   w.bytes = off;
   return w;
 }
@@ -476,20 +475,12 @@ int ws_strct_bits(const uint8_t* st, int64_t odz, int64_t ody, int64_t odx, uint
   return B2V_OK;
 }
 
-int ws_grid(int64_t n) {
-  int64_t blocks = ceil_div64(n, 256 * 4);
-  int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 }  // namespace
 
 extern "C" int b2v_ws_lut_i16(const int16_t* img, int64_t n, double window, double level, uint16_t* out,
                               void* stream) {
   B2V_REQUIRE(img && out && n > 0, B2V_ERR_ARG, "ws_lut: bad arguments");
-  k_ws_lut<<<ws_grid(n), 256, 0, (cudaStream_t)stream>>>(img, n, window, level, out);
+  k_ws_lut<<<b2v_grid(n, 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(img, n, window, level, out);
   return b2v_check_launch("k_ws_lut");
 }
 
@@ -498,13 +489,13 @@ extern "C" int b2v_ws_shift_i16(const int16_t* img, int64_t n, uint16_t* out, vo
   float* mm = (float*)workspace;
   int rc = b2v_minmax_f32(img, B2V_I16, n, mm, (char*)workspace + 256, stream);
   if (rc) return rc;
-  k_ws_shift<<<ws_grid(n), 256, 0, (cudaStream_t)stream>>>(img, n, mm, out);
+  k_ws_shift<<<b2v_grid(n, 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(img, n, mm, out);
   return b2v_check_launch("k_ws_shift");
 }
 
 extern "C" int b2v_ws_shift_i16_with(const int16_t* img, int64_t n, const float* minmax_dev, uint16_t* out, void* stream) {
   B2V_REQUIRE(img && out && minmax_dev && n > 0, B2V_ERR_ARG, "ws_shift: bad arguments");
-  k_ws_shift<<<ws_grid(n), 256, 0, (cudaStream_t)stream>>>(img, n, minmax_dev, out);
+  k_ws_shift<<<b2v_grid(n, 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(img, n, minmax_dev, out);
   return b2v_check_launch("k_ws_shift");
 }
 
@@ -530,7 +521,8 @@ extern "C" int b2v_ws_morph_gradient_u16(const uint16_t* in, int64_t nz, int64_t
 #undef B2V_MG
     return b2v_check_launch("k_ws_morph_gradient_cols");
   }
-  k_ws_morph_gradient<<<ws_grid(nz * ny * nx), 256, 0, (cudaStream_t)stream>>>(in, nz, ny, nx, sz, sy, sx, out);
+  k_ws_morph_gradient<<<b2v_grid(nz * ny * nx, 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(in, nz, ny, nx, sz, sy, sx,
+                                                                                             out);
   return b2v_check_launch("k_ws_morph_gradient");
 }
 
@@ -572,7 +564,8 @@ extern "C" int b2v_ws_flood(const uint16_t* img, const int16_t* markers, int64_t
   const int64_t n = nz * ny * nx;
   const int64_t ntiles = (int64_t)g.ntz * g.nty * g.ntx;
   B2V_CUDA(cudaMemsetAsync(w.active[0], 0, (size_t)((char*)w.flags - (char*)w.active[0]) + (kMaxRounds + 2) * 4, s));
-  k_ws_init<<<ws_grid(n), 256, 0, s>>>(img, markers, g, mode, w.cost, w.key, w.lset, w.active[0], w.flags);
+  k_ws_init<<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>(img, markers, g, mode, w.cost, w.key, w.lset, w.active[0],
+                                                     w.flags);
   if ((rc = b2v_check_launch("k_ws_init"))) return rc;
   int round = 0;
   rc = mode == 0 ? run_phase<1, 0>(img, w, g, sb, s, &round) : run_phase<1, 1>(img, w, g, sb, s, &round);
@@ -582,7 +575,7 @@ extern "C" int b2v_ws_flood(const uint16_t* img, const int16_t* markers, int64_t
   if ((rc = b2v_check_launch("k_ws_activate_all"))) return rc;
   rc = mode == 0 ? run_phase<2, 0>(img, w, g, sb, s, &round) : run_phase<2, 1>(img, w, g, sb, s, &round);
   if (rc) return rc;
-  k_ws_labels<<<ws_grid(n), 256, 0, s>>>(w.key, w.lset, n, labels, ambiguous);
+  k_ws_labels<<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>(w.key, w.lset, n, labels, ambiguous);
   if ((rc = b2v_check_launch("k_ws_labels"))) return rc;
   if (rounds_out) *rounds_out = round;
   return B2V_OK;

@@ -100,27 +100,26 @@ FGrid make_fgrid(int64_t nz, int64_t ny, int64_t nx, int mode, int frozen_lo, in
 
 FastWs fcarve(void* base, int64_t nz, int64_t ny, int64_t nx) {
   FastWs w;
-  auto align = [](int64_t v) { return (v + 255) & ~(int64_t)255; };
   const int64_t n = nz * ny * nx;
   const int64_t nt = ceil_div64(nz, kT) * ceil_div64(ny, kT) * ceil_div64(nx, kT);
   const int64_t nbw = (nt + 31) / 32;
   char* p = (char*)base;
   int64_t off = 0;
-  w.key = (unsigned long long*)(p + off); off += align(n * 8);
-  w.cost = (uint32_t*)(p + off); off += align(n * 4);
-  w.lset = (uint16_t*)(p + off); off += align(n * 2);
-  w.adm = (uint8_t*)(p + off); off += align(n);
-  w.key32 = (uint32_t*)(p + off); off += align(n * 4);
+  w.key = (unsigned long long*)(p + off); off += align256(n * 8);
+  w.cost = (uint32_t*)(p + off); off += align256(n * 4);
+  w.lset = (uint16_t*)(p + off); off += align256(n * 2);
+  w.adm = (uint8_t*)(p + off); off += align256(n);
+  w.key32 = (uint32_t*)(p + off); off += align256(n * 4);
   w.present = (uint32_t*)(p + off); off += 2048 * 4;
   w.prefix = (uint32_t*)(p + off); off += 2048 * 4;
-  w.inv = (uint32_t*)(p + off); off += align(257 * 4);
-  w.init_list = (int*)(p + off); off += align(nt * 4);
+  w.inv = (uint32_t*)(p + off); off += align256(257 * 4);
+  w.init_list = (int*)(p + off); off += align256(nt * 4);
   w.init_cnt = (int*)(p + off); off += 256;
   w.lists_begin = p + off;
-  w.L.bm = (uint32_t*)(p + off); off += align(3 * nbw * 4);
+  w.L.bm = (uint32_t*)(p + off); off += align256(3 * nbw * 4);
   w.L.cnt = (int*)(p + off); off += 256;
   w.lists_bytes = (p + off) - w.lists_begin;
-  w.L.list = (int*)(p + off); off += align(3 * nt * 4);
+  w.L.list = (int*)(p + off); off += align256(3 * nt * 4);
   w.L.nbw = (int)nbw;
   w.bytes = off;
   return w;
@@ -941,14 +940,6 @@ __global__ void __launch_bounds__(256) k_wsf_plane_merge(uint32_t* cost, unsigne
   }
 }
 
-int wsf_grid(long long n) {
-  long long blocks = ceil_div64(n, 256 * 4);
-  long long cap = (long long)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
 template <typename K>
 int launch_persistent(K kern, size_t smem, const uint16_t* img, FastWs& w, FGrid g, cudaStream_t s, void* keyptr = nullptr) {
   B2V_CUDA(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1005,8 +996,8 @@ int b2v_wsf_run(int stages, const uint16_t* img, const int16_t* markers, int64_t
     B2V_REQUIRE(markers, B2V_ERR_ARG, "ws_flood: null markers");
     B2V_CUDA(cudaMemsetAsync(w.init_cnt, 0, 256 + (size_t)w.lists_bytes, s));
     B2V_CUDA(cudaMemsetAsync(w.present, 0, 2048 * 4, s));
-    k_wsf_init<<<wsf_grid(g.n), 256, 0, s>>>(img, markers, g, w.cost, w.key, w.lset, w.L, w.init_list, w.init_cnt,
-                                             w.present);
+    k_wsf_init<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(img, markers, g, w.cost, w.key, w.lset, w.L, w.init_list,
+                                                          w.init_cnt, w.present);
     if ((rc = b2v_check_launch("k_wsf_init"))) return rc;
     k_wsf_ranks<<<1, 1024, 0, s>>>(w.present, w.prefix, w.inv);
     if ((rc = b2v_check_launch("k_wsf_ranks"))) return rc;
@@ -1030,13 +1021,13 @@ int b2v_wsf_run(int stages, const uint16_t* img, const int16_t* markers, int64_t
   }
   if (stages & 4) {
     B2V_CUDA(cudaMemsetAsync(w.lists_begin, 0, (size_t)w.lists_bytes, s));
-    k_wsf_adm<<<wsf_grid(g.n), 256, 0, s>>>(img, w.cost, w.key, g, w.adm);
+    k_wsf_adm<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(img, w.cost, w.key, g, w.adm);
     if ((rc = b2v_check_launch("k_wsf_adm"))) return rc;
     k_wsf_seed_lists<<<8, 256, 0, s>>>(w.L, w.init_list, w.init_cnt);
     if ((rc = b2v_check_launch("k_wsf_seed_lists"))) return rc;
   }
   if ((stages & 8) && use32) {
-    k_wsf_key32_init<<<wsf_grid(g.n), 256, 0, s>>>(w.key, g.n, w.present, w.prefix, w.key32);
+    k_wsf_key32_init<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(w.key, g.n, w.present, w.prefix, w.key32);
     if ((rc = b2v_check_launch("k_wsf_key32_init"))) return rc;
     const size_t smem = (size_t)kCells * (with_set ? 7 : 5) + 16;
     rc = with_set ? launch_persistent(k_wsf_persistent<2, 0, true, uint32_t>, smem, img, w, g, s, w.key32)
@@ -1062,8 +1053,9 @@ int b2v_wsf_run(int stages, const uint16_t* img, const int16_t* markers, int64_t
   if (stages & 16) {
     B2V_REQUIRE(labels, B2V_ERR_ARG, "ws_flood: null labels");
     B2V_REQUIRE(!ambiguous || with_set, B2V_ERR_ARG, "ws_flood: the ambiguous mask needs the label sets");
-    if (use32) k_wsf_labels32<<<wsf_grid(g.n), 256, 0, s>>>(w.key32, w.lset, w.inv, g.n, labels, ambiguous);
-    else k_wsf_labels<<<wsf_grid(g.n), 256, 0, s>>>(w.key, w.lset, g.n, labels, ambiguous);
+    if (use32) k_wsf_labels32<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(w.key32, w.lset, w.inv, g.n, labels,
+                                                                         ambiguous);
+    else k_wsf_labels<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(w.key, w.lset, g.n, labels, ambiguous);
     if ((rc = b2v_check_launch("k_wsf_labels"))) return rc;
   }
   return B2V_OK;

@@ -521,10 +521,7 @@ int prefilter_volume(const void* in, int in_dtype, int64_t nz, int64_t ny, int64
 template <typename T, int ORDER>
 int gather_launch(const void* src, const GatherParams& P, void* out, cudaStream_t s) {
   const int64_t total = P.ax[0].n_out * P.ax[1].n_out * P.ax[2].n_out;
-  int64_t blocks = ceil_div64(total, 256);
-  const int64_t cap = (int64_t)b2v_sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  k_zoom_gather<T, ORDER><<<(unsigned)blocks, 256, 0, s>>>((const T*)src, P, out);
+  k_zoom_gather<T, ORDER><<<b2v_grid(total, 256, 16), 256, 0, s>>>((const T*)src, P, out);
   return b2v_check_launch("k_zoom_gather");
 }
 

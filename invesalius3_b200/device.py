@@ -52,6 +52,51 @@ def _workspace(nbytes: int, device) -> torch.Tensor | None:
     return torch.empty(int(nbytes), dtype=torch.uint8, device=device) if nbytes > 0 else None
 
 
+# ----------------------------------------------------------------------------- triangle meshes
+# vertices float32 [V,3]; faces int32 / int64 [T,3], or [T,4] with a leading 3 (the Mesh form)
+def _face_form(shape) -> int:
+    if len(shape) != 2 or shape[1] not in (3, 4):
+        raise ValueError("faces: [T,3] or [T,4] (leading 3) expected")
+    return int(shape[1])
+
+
+def _mesh_tensors(vertices, faces, caller: str) -> int:
+    """Checks a mesh given as dense CUDA tensors on one device; returns the face form (3 or 4 columns)."""
+    if not isinstance(vertices, torch.Tensor) or not isinstance(faces, torch.Tensor):
+        raise TypeError(f"{caller}: torch tensors expected")
+    if vertices.dtype != torch.float32:
+        raise TypeError("vertices: float32 expected")
+    if faces.dtype not in (torch.int32, torch.int64):
+        raise TypeError("faces: int32 or int64 expected")
+    if vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError("vertices: [V,3] expected")
+    cols = _face_form(tuple(faces.shape))
+    _dense(vertices, "vertices")
+    _dense(faces, "faces")
+    if faces.device != vertices.device:
+        raise ValueError("vertices and faces must be on the same device")
+    return cols
+
+
+def _mesh_arrays(vertices, faces) -> int:
+    """Checks a mesh given as numpy arrays; returns the face form (3 or 4 columns)."""
+    if not isinstance(vertices, np.ndarray) or vertices.dtype != np.float32:
+        raise TypeError("vertices: a float32 numpy array expected")
+    if not isinstance(faces, np.ndarray) or faces.dtype not in (np.int32, np.int64):
+        raise TypeError("faces: an int32 or int64 numpy array expected")
+    if vertices.ndim != 2 or vertices.shape[1] != 3:
+        raise ValueError("vertices: [V,3] expected")
+    return _face_form(faces.shape)
+
+
+def _as_form(f32: torch.Tensor, dtype: torch.dtype, cols: int) -> torch.Tensor:
+    """int32 [T,3] device faces in the given dtype and form."""
+    f = f32 if dtype == torch.int32 else f32.to(dtype)
+    if cols == 4:
+        f = torch.cat((torch.full((f.shape[0], 1), 3, dtype=dtype, device=f.device), f), 1)
+    return f
+
+
 # ----------------------------------------------------------------------------- transfers
 def _box_pitches(a: np.ndarray):
     """(row_pitch, plane_pitch) in bytes if `a` (3-D) is an x-contiguous box view."""

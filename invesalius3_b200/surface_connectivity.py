@@ -28,8 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .device import _dense, _p, _stream, _workspace, require_cuda
-from .visible_faces import _as_form, _face_form
+from .device import _as_form, _mesh_arrays, _mesh_tensors, _p, _stream, _workspace, require_cuda
 
 
 @dataclass
@@ -54,23 +53,6 @@ class Connectivity:
     depth: int
 
 
-def _check(vertices, faces):
-    if not isinstance(vertices, torch.Tensor) or not isinstance(faces, torch.Tensor):
-        raise TypeError("connectivity: torch tensors expected")
-    if vertices.dtype != torch.float32:
-        raise TypeError("vertices: float32 expected")
-    if faces.dtype not in (torch.int32, torch.int64):
-        raise TypeError("faces: int32 or int64 expected")
-    if vertices.dim() != 2 or vertices.shape[1] != 3:
-        raise ValueError("vertices: [V,3] expected")
-    cols = _face_form(tuple(faces.shape), "faces")
-    _dense(vertices, "vertices")
-    _dense(faces, "faces")
-    if faces.device != vertices.device:
-        raise ValueError("vertices and faces must be on the same device")
-    return cols
-
-
 def _seeds(seeds) -> np.ndarray:
     try:
         s = np.asarray(seeds, dtype=np.int64).reshape(-1)
@@ -82,7 +64,7 @@ def _seeds(seeds) -> np.ndarray:
 def connectivity_device(vertices: torch.Tensor, faces: torch.Tensor, seeds=None) -> Connectivity:
     """Runs the filter: every region (seeds=None) or the region grown from the point ids `seeds`.
     Synchronises: the counts come back to the host."""
-    cols = _check(vertices, faces)
+    cols = _mesh_tensors(vertices, faces, "connectivity")
     nv, nt, dev = vertices.shape[0], faces.shape[0], vertices.device
     s = None if seeds is None else _seeds(seeds)
     ns = 0 if s is None else len(s)
@@ -153,7 +135,7 @@ def _largest_offsets(c: Connectivity):
 def select_largest_part_device(vertices: torch.Tensor, faces: torch.Tensor, compact: bool = False):
     """polydata_utils.SelectLargestPart on device tensors: (vertices, faces, point_ids, cell_ids), the ids
     int32."""
-    cols = _check(vertices, faces)
+    cols = _mesh_tensors(vertices, faces, "connectivity")
     c = connectivity_device(vertices, faces)
     return _part(c, *_largest_offsets(c), faces.dtype, cols, compact)
 
@@ -162,7 +144,7 @@ def split_disconnected_parts_device(vertices: torch.Tensor, faces: torch.Tensor,
     """polydata_utils.SplitDisconectedParts on device tensors: one (vertices, faces, point_ids, cell_ids) per
     region, in region order; one traversal serves them all. In the VTK form every part's vertices and
     point_ids are the same tensors."""
-    cols = _check(vertices, faces)
+    cols = _mesh_tensors(vertices, faces, "connectivity")
     c = connectivity_device(vertices, faces)
     poff, coff = c.point_offsets.tolist(), c.cell_offsets.tolist()
     return [_part(c, r, poff, coff, faces.dtype, cols, compact) for r in range(len(coff) - 1)]
@@ -171,20 +153,14 @@ def split_disconnected_parts_device(vertices: torch.Tensor, faces: torch.Tensor,
 def join_seeds_parts_device(vertices: torch.Tensor, faces: torch.Tensor, seeds, compact: bool = False):
     """polydata_utils.JoinSeedsParts on device tensors: (vertices, faces, point_ids, cell_ids) of the faces
     reached from the point ids `seeds`."""
-    cols = _check(vertices, faces)
+    cols = _mesh_tensors(vertices, faces, "connectivity")
     c = connectivity_device(vertices, faces, seeds)
     return _part(c, None, None, None, faces.dtype, cols, compact)
 
 
 def _on_host(vertices, faces, seeds=None):
     """connectivity_device on numpy arrays, its result copied to the host once."""
-    if not isinstance(vertices, np.ndarray) or vertices.dtype != np.float32:
-        raise TypeError("vertices: a float32 numpy array expected")
-    if not isinstance(faces, np.ndarray) or faces.dtype not in (np.int32, np.int64):
-        raise TypeError("faces: an int32 or int64 numpy array expected")
-    if vertices.ndim != 2 or vertices.shape[1] != 3:
-        raise ValueError("vertices: [V,3] expected")
-    cols = _face_form(faces.shape, "faces")
+    cols = _mesh_arrays(vertices, faces)
     require_cuda()
     c = connectivity_device(torch.from_numpy(np.ascontiguousarray(vertices)).cuda(),
                             torch.from_numpy(np.ascontiguousarray(faces)).cuda(), seeds)

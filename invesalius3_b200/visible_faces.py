@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .device import _dense, _p, _stream, _workspace, require_cuda
+from .device import _as_form, _mesh_arrays, _mesh_tensors, _p, _stream, _workspace, require_cuda
 
 DEFAULT_POSITIONS = ((1, 0, 0), (-1, 0, 0), (0, 1, 0), (0, -1, 0), (0, 0, 1), (0, 0, -1))
 MAX_VIEWS = 64
@@ -42,39 +42,14 @@ def _positions(positions) -> np.ndarray:
     return np.ascontiguousarray(p)
 
 
-def _face_form(shape, what: str) -> int:
-    if len(shape) != 2 or shape[1] not in (3, 4):
-        raise ValueError(f"{what}: [T,3] or [T,4] (leading 3) expected")
-    return int(shape[1])
-
-
-def _as_form(f32: torch.Tensor, dtype: torch.dtype, cols: int) -> torch.Tensor:
-    f = f32 if dtype == torch.int32 else f32.to(dtype)
-    if cols == 4:
-        f = torch.cat((torch.full((f.shape[0], 1), 3, dtype=dtype, device=f.device), f), 1)
-    return f
-
-
 def remove_non_visible_faces_device(vertices: torch.Tensor, faces: torch.Tensor, positions=DEFAULT_POSITIONS,
                                     remove_visible: bool = False, _debug: dict | None = None):
     """(vertices float32 [V',3], faces [T',3|4]) device tensors. Synchronises twice: the vertex bounds and
     the output counts come back to the host. _debug, if a dict, receives the bounds, the camera records,
     and views into the workspace of the depth buffers, the per-vertex visibility and the number of
     triangles the cooperative (large-triangle) path drew."""
-    if not isinstance(vertices, torch.Tensor) or not isinstance(faces, torch.Tensor):
-        raise TypeError("remove_non_visible_faces_device: torch tensors expected")
-    if vertices.dtype != torch.float32:
-        raise TypeError("vertices: float32 expected")
-    if faces.dtype not in (torch.int32, torch.int64):
-        raise TypeError("faces: int32 or int64 expected")
-    if vertices.dim() != 2 or vertices.shape[1] != 3:
-        raise ValueError("vertices: [V,3] expected")
-    cols = _face_form(tuple(faces.shape), "faces")
+    cols = _mesh_tensors(vertices, faces, "remove_non_visible_faces_device")
     p = _positions(positions)
-    _dense(vertices, "vertices")
-    _dense(faces, "faces")
-    if faces.device != vertices.device:
-        raise ValueError("vertices and faces must be on the same device")
     nv, nt, nviews = vertices.shape[0], faces.shape[0], len(p)
     dev = vertices.device
     if nv == 0:
@@ -112,13 +87,7 @@ def remove_non_visible_faces_device(vertices: torch.Tensor, faces: torch.Tensor,
 def remove_non_visible_faces(vertices, faces, positions=DEFAULT_POSITIONS, remove_visible: bool = False):
     """The plugin's remove_non_visible_faces(polydata, positions, remove_visible) on arrays: returns
     (vertices float32 [V',3], faces) with faces in the input's dtype and form."""
-    if not isinstance(vertices, np.ndarray) or vertices.dtype != np.float32:
-        raise TypeError("vertices: a float32 numpy array expected")
-    if not isinstance(faces, np.ndarray) or faces.dtype not in (np.int32, np.int64):
-        raise TypeError("faces: an int32 or int64 numpy array expected")
-    if vertices.ndim != 2 or vertices.shape[1] != 3:
-        raise ValueError("vertices: [V,3] expected")
-    cols = _face_form(faces.shape, "faces")
+    cols = _mesh_arrays(vertices, faces)
     _positions(positions)
     if not np.isfinite(vertices).all():
         raise ValueError("vertices must be finite")
