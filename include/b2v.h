@@ -501,6 +501,35 @@ int b2v_conn_emit(const float* verts, int64_t nv, int64_t nt, int64_t nseeds, co
                   void* workspace, float* verts_out, int32_t* point_ids, int32_t* faces_out, int32_t* cell_ids,
                   int64_t* point_offsets, int64_t* cell_offsets, void* stream);
 
+/* ---- surface smoothing ---------------------------------------------------------------------------
+ * vtkSmoothPolyDataFilter (Laplacian, in place in ascending point id) on triangles, behind
+ * polydata_utils.ApplySmoothFilter, surface.decimate_polydata and markers/surface_geometry. The contract
+ * (VTK's edge analysis, vertex types, sweep order and early stop, restated and unverified) is in DESIGN.md §3
+ * and the header of the C checker, smoothing.c. The result equals the sequential sweep bit for bit.
+ *   verts: float32 [nv][3]; faces: int32 (faces_i64 = 0) or int64 [nt][face_cols], face_cols 3, or 4 with a
+ *   leading 3 in every row; nv < 2^31, 6 nt < 2^32. A bad face is B2V_ERR_ARG.
+ *   b2v_smooth_analyse  edge analysis, vertex types and edge lists, and the dependency levels of the sweep.
+ *                       cos_feature / cos_edge: the cosines of the feature and edge angles.
+ *                       bounds_host[6] = {xmin, xmax, ymin, ymax, zmin, zmax} of the points the faces use
+ *                       (0 without faces); counts_host[3] = {movable points, levels, grid barriers}.
+ *                       Synchronises the stream.
+ *   b2v_smooth_run      from the same workspace: verts_out float32 [nv][3] = the smoothed points (verts is
+ *                       not modified). The sweep stops after `iterations` iterations, or after the first
+ *                       whose largest move is <= conv (an absolute distance). counts_host[3] = {iterations
+ *                       done, steps (levels x iterations done), grid barriers}. Synchronises the stream.
+ *   b2v_smooth_layout   byte offsets in the workspace, valid after the analysis: [0] int8 [nv] vertex types
+ *                       (VTK's codes: 0 simple, 1 fixed, 2 feature edge, 3 boundary edge), [1] int32 [nv]
+ *                       edge-list lengths, [2] uint64 [nv + 1] where each point's list starts in [3] int32
+ *                       [6 nt], [4] int32 [movable] the movable points level by level, [5] uint64
+ *                       [levels + 1] the level offsets. */
+int64_t b2v_smooth_workspace_bytes(int64_t nv, int64_t nt);
+int b2v_smooth_layout(int64_t nv, int64_t nt, int64_t* layout_out);
+int b2v_smooth_analyse(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                       double cos_feature, double cos_edge, int feature_edge_smoothing, int boundary_smoothing,
+                       void* workspace, void* stream, double* bounds_host, int64_t* counts_host);
+int b2v_smooth_run(const float* verts, int64_t nv, int64_t nt, int64_t iterations, double relaxation, double conv,
+                   void* workspace, float* verts_out, void* stream, int64_t* counts_host);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

@@ -1,0 +1,181 @@
+// The point -> cell links of a triangle mesh (vtkCellLinks), and the device-wide scan and stable radix sort
+// they are built with. Shared by the surface tools that walk a mesh through its links (connectivity.cu,
+// smoothing.cu); every name is in an anonymous namespace, so each translation unit has its own copy.
+//
+//   k_conn_load   faces -> int32 [T][3] (a bad face sets ST_BAD_FACE), link counts per point.
+//   lstart        an exclusive scan of the counts: point p's links are links[lstart[p], lstart[p + 1]).
+//   links         the corners (in corner order, i.e. ascending cell) stably sorted by point id: each point's
+//                 cells in ascending id, a degenerate triangle once per corner it occupies.
+//
+// Stable sorts are LSD radix passes of 8 bits (per-block digit histograms, one scan, a scatter ranked by
+// warp match), only over the bits the largest key needs.
+#pragma once
+#include "b2v_common.cuh"
+
+namespace {
+
+constexpr int kBlock = 256;
+constexpr int kScanItems = 4;                      // items per thread of the device-wide scan
+constexpr int kScanTile = kBlock * kScanItems;
+
+int64_t scan_blocks(int64_t n) { return ceil_div64(n > 0 ? n : 1, kScanTile); }
+
+// ---- device-wide exclusive scan of uint64 in place (tiles of kScanTile, then the tile sums) ----------------
+__global__ void __launch_bounds__(kBlock) k_scan_tiles(unsigned long long* a, int64_t n,
+                                                       unsigned long long* sums) {
+  __shared__ unsigned long long s_w[kBlock / 32];
+  const int64_t base = (int64_t)blockIdx.x * kScanTile + (int64_t)threadIdx.x * kScanItems;
+  unsigned long long v[kScanItems], s = 0;
+  for (int k = 0; k < kScanItems; ++k) {
+    v[k] = base + k < n ? a[base + k] : 0ull;
+    s += v[k];
+  }
+  unsigned long long tot;
+  unsigned long long ex = block_exscan<unsigned long long>(s, s_w, &tot);
+  for (int k = 0; k < kScanItems; ++k) {
+    if (base + k < n) a[base + k] = ex;
+    ex += v[k];
+  }
+  if (threadIdx.x == 0) sums[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(1024) k_scan_sums(unsigned long long* a, int64_t nb, unsigned long long* total) {
+  __shared__ unsigned long long s_w[32];
+  unsigned long long carry = 0;
+  for (int64_t base = 0; base < nb; base += blockDim.x) {
+    const int64_t i = base + threadIdx.x;
+    const unsigned long long x = i < nb ? a[i] : 0ull;
+    unsigned long long tot;
+    const unsigned long long ex = block_exscan<unsigned long long>(x, s_w, &tot);
+    if (i < nb) a[i] = carry + ex;
+    carry += tot;
+  }
+  if (threadIdx.x == 0 && total) *total = carry;
+}
+
+__global__ void __launch_bounds__(kBlock) k_scan_add(unsigned long long* a, int64_t n,
+                                                     const unsigned long long* __restrict__ sums) {
+  const unsigned long long add = sums[blockIdx.x];
+  const int64_t base = (int64_t)blockIdx.x * kScanTile;
+  for (int k = threadIdx.x; k < kScanTile; k += kBlock)
+    if (base + k < n) a[base + k] += add;
+}
+
+// scratch: scan_blocks(n) + 1 words; total (may be null): the sum of a[0, n), written on the device
+int scan(unsigned long long* a, int64_t n, unsigned long long* scratch, unsigned long long* total, cudaStream_t s) {
+  const int64_t nb = scan_blocks(n);
+  B2V_REQUIRE(nb <= 0x7fffffffLL, B2V_ERR_ARG, "scan too long");
+  k_scan_tiles<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
+  if (int rc = b2v_check_launch("k_scan_tiles")) return rc;
+  k_scan_sums<<<1, 1024, 0, s>>>(scratch, nb, total);
+  if (int rc = b2v_check_launch("k_scan_sums")) return rc;
+  k_scan_add<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
+  return b2v_check_launch("k_scan_add");
+}
+
+// ---- stable LSD radix sort of (key, value) pairs, 8 bits a pass -------------------------------------------
+__global__ void __launch_bounds__(kBlock) k_rs_hist(const uint32_t* __restrict__ keys, int64_t n, int shift,
+                                                    int64_t nb, unsigned long long* hist) {
+  __shared__ uint32_t s_c[256];
+  s_c[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i < n) atomicAdd(&s_c[(keys[i] >> shift) & 255u], 1u);
+  __syncthreads();
+  hist[(int64_t)threadIdx.x * nb + blockIdx.x] = s_c[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(kBlock) k_rs_scatter(const uint32_t* __restrict__ kin,
+                                                       const uint32_t* __restrict__ vin, int64_t n, int shift,
+                                                       int64_t nb, const unsigned long long* __restrict__ hist,
+                                                       uint32_t* __restrict__ kout, uint32_t* __restrict__ vout) {
+  __shared__ uint32_t s_c[kBlock / 32][256];
+  for (int k = threadIdx.x; k < (kBlock / 32) * 256; k += kBlock) (&s_c[0][0])[k] = 0;
+  __syncthreads();
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t key = i < n ? kin[i] : 0u;
+  const uint32_t d = i < n ? (key >> shift) & 255u : 256u;   // 256: no item
+  const uint32_t peers = __match_any_sync(0xffffffffu, d);
+  const uint32_t below = peers & ((1u << lane) - 1u);
+  if (d < 256u && below == 0) s_c[wid][d] = __popc(peers);
+  __syncthreads();
+  if (d >= 256u) return;
+  uint32_t r = __popc(below);
+  for (int w = 0; w < wid; ++w) r += s_c[w][d];
+  const unsigned long long pos = hist[(int64_t)d * nb + blockIdx.x] + r;
+  kout[pos] = key;
+  vout[pos] = vin[i];
+}
+
+// Sorts (w.ka, w.va)[0..n) stably by key < 2^keybits; the result is in (ka, va) or (kb, vb): *out_v says
+// which. W is a workspace record with the four [n] ping-pong arrays ka, va, kb, vb, hist
+// [256 ceil(n / kBlock) + 1] and scratch [scan_blocks(that) + 1].
+template <typename W>
+int sort_pairs(W& w, int64_t n, int keybits, uint32_t** out_v, cudaStream_t s) {
+  uint32_t *ki = w.ka, *vi = w.va, *ko = w.kb, *vo = w.vb;
+  const int64_t nb = ceil_div64(n, kBlock);
+  for (int shift = 0; shift < keybits && n > 1; shift += 8) {
+    k_rs_hist<<<(unsigned)nb, kBlock, 0, s>>>(ki, n, shift, nb, w.hist);
+    if (int rc = b2v_check_launch("k_rs_hist")) return rc;
+    if (int rc = scan(w.hist, 256 * nb, w.scratch, nullptr, s)) return rc;
+    k_rs_scatter<<<(unsigned)nb, kBlock, 0, s>>>(ki, vi, n, shift, nb, w.hist, ko, vo);
+    if (int rc = b2v_check_launch("k_rs_scatter")) return rc;
+    uint32_t* t = ki; ki = ko; ko = t;
+    t = vi; vi = vo; vo = t;
+  }
+  *out_v = vi;
+  return B2V_OK;
+}
+
+int bits_for(int64_t max_key) {
+  int b = 0;
+  while (b < 32 && (max_key >> b) > 0) ++b;
+  return b;
+}
+
+// ---- faces and links -------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kBlock) k_conn_load(Faces F, int32_t* __restrict__ tri, unsigned long long* deg,
+                                                     uint32_t* ka, uint32_t* va, uint32_t* status) {
+  for (int64_t t = gtid(); t < F.nt; t += gstride()) {
+    int64_t v[3];
+    if (!load_face(F, t, v)) {
+      atomicOr(status, ST_BAD_FACE);
+      v[0] = v[1] = v[2] = 0;
+    }
+    for (int j = 0; j < 3; ++j) {
+      tri[3 * t + j] = (int32_t)v[j];
+      atomicAdd(&deg[v[j]], 1ull);
+      ka[3 * t + j] = (uint32_t)v[j];
+      va[3 * t + j] = (uint32_t)t;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_copy_i32(const uint32_t* __restrict__ in, int64_t n, int32_t* out) {
+  for (int64_t i = gtid(); i < n; i += gstride()) out[i] = (int32_t)in[i];
+}
+
+// Loads the faces into w.tri and builds w.lstart [V + 1] and w.links [3T] (nt > 0). W also holds status and
+// the sort buffers of sort_pairs, with room for 3T items. A bad face is B2V_ERR_ARG, reported as
+// "<what>: a face has an index ...". Synchronises the stream.
+template <typename W>
+int build_links(W& w, const Faces& F, const char* what, cudaStream_t s) {
+  const int64_t nv = F.nv, C3 = 3 * F.nt;
+  B2V_CUDA(cudaMemsetAsync(w.status, 0, 16, s));
+  B2V_CUDA(cudaMemsetAsync(w.lstart, 0, (size_t)(nv + 1) * 8, s));
+  k_conn_load<<<b2v_grid(F.nt, kBlock, 16), kBlock, 0, s>>>(F, w.tri, w.lstart, w.ka, w.va, w.status);
+  if (int rc = b2v_check_launch("k_conn_load")) return rc;
+  uint32_t status = 0;
+  B2V_CUDA(cudaMemcpyAsync(&status, w.status, 4, cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaStreamSynchronize(s));
+  B2V_REQUIRE(!(status & ST_BAD_FACE), B2V_ERR_ARG,
+              "%s: a face has an index outside [0, V) (or a leading entry other than 3)", what);
+  if (int rc = scan(w.lstart, nv + 1, w.scratch, nullptr, s)) return rc;
+  uint32_t* lv = nullptr;
+  if (int rc = sort_pairs(w, C3, bits_for(nv - 1), &lv, s)) return rc;
+  k_copy_i32<<<b2v_grid(C3, kBlock, 16), kBlock, 0, s>>>(lv, C3, w.links);
+  return b2v_check_launch("k_copy_i32");
+}
+
+}  // namespace
