@@ -530,6 +530,31 @@ int b2v_smooth_analyse(const float* verts, int64_t nv, const void* faces, int64_
 int b2v_smooth_run(const float* verts, int64_t nv, int64_t nt, int64_t iterations, double relaxation, double conv,
                    void* workspace, float* verts_out, void* stream, int64_t* counts_host);
 
+/* ---- surface hole filling -------------------------------------------------------------------------
+ * vtkFillHolesFilter on triangles, behind polydata_utils.ApplySmoothFilter, surface_process's "Fill holes",
+ * FillSurfaceHole and markers/surface_geometry. The contract (boundary lines, the loop tracing, the bounding-
+ * sphere test and the ear-clipping rule, restated and unverified) is in DESIGN.md §3 and the header of the C
+ * checker, fill_holes.c. The result equals the sequential filter bit for bit.
+ *   verts: float32 [nv][3]; faces: int32 (faces_i64 = 0) or int64 [nt][face_cols], face_cols 3, or 4 with a
+ *   leading 3 in every row; nv < 2^31, 6 nt < 2^31. A bad face is B2V_ERR_ARG.
+ *   b2v_holes_count   finds, traces, sizes and triangulates the holes. hole_size: NaN is B2V_ERR_ARG, other
+ *                     values are clamped to [0, FLT_MAX]. counts_host[3] = {boundary lines, loops, new
+ *                     triangles}. Synchronises the stream.
+ *   b2v_holes_emit    from the same workspace: faces_out [nt + new triangles][face_cols] in the input's dtype
+ *                     and form, the input faces first; per loop, in the order of its first line: first_line
+ *                     and npts (int64), radius (double) and status (int8: 0 filled, 1 failed, 2 too large).
+ *                     Does not synchronise.
+ *   b2v_holes_layout  byte offsets in the workspace, valid after the count: [0] int32 [lines][2] the boundary
+ *                     lines, [1] int32 [points] the loops' points, loop after loop, [2] uint64 [loops] where
+ *                     each loop starts in [1], [3] int32 [loops] its points. */
+int64_t b2v_holes_workspace_bytes(int64_t nv, int64_t nt);
+int b2v_holes_layout(int64_t nv, int64_t nt, int64_t* layout_out);
+int b2v_holes_count(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                    double hole_size, void* workspace, void* stream, int64_t* counts_host);
+int b2v_holes_emit(const void* faces, int64_t nv, int64_t nt, int face_cols, int faces_i64,
+                   const int64_t* counts_host, void* workspace, void* faces_out, int64_t* first_line,
+                   int64_t* npts, double* radius, int8_t* status, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

@@ -138,6 +138,10 @@ PROTOTYPES = {
     "b2v_smooth_analyse": (cint, [vp, i64, vp, i64, cint, cint, dbl, dbl, cint, cint, vp, vp, C.POINTER(dbl),
                                   C.POINTER(i64)]),
     "b2v_smooth_run": (cint, [vp, i64, i64, i64, dbl, dbl, vp, vp, vp, C.POINTER(i64)]),
+    "b2v_holes_workspace_bytes": (i64, [i64, i64]),
+    "b2v_holes_layout": (cint, [i64, i64, C.POINTER(i64)]),
+    "b2v_holes_count": (cint, [vp, i64, vp, i64, cint, cint, dbl, vp, vp, C.POINTER(i64)]),
+    "b2v_holes_emit": (cint, [vp, i64, i64, cint, cint, C.POINTER(i64), vp, vp, vp, vp, vp, vp, vp]),
 }
 
 VIS_CAMERA_DOUBLES = 32

@@ -1,11 +1,13 @@
 // The point -> cell links of a triangle mesh (vtkCellLinks), and the device-wide scan and stable radix sort
 // they are built with. Shared by the surface tools that walk a mesh through its links (connectivity.cu,
-// smoothing.cu); every name is in an anonymous namespace, so each translation unit has its own copy.
+// smoothing.cu, fill_holes.cu); every name is in an anonymous namespace, so each translation unit has its own
+// copy.
 //
 //   k_conn_load   faces -> int32 [T][3] (a bad face sets ST_BAD_FACE), link counts per point.
 //   lstart        an exclusive scan of the counts: point p's links are links[lstart[p], lstart[p + 1]).
 //   links         the corners (in corner order, i.e. ascending cell) stably sorted by point id: each point's
 //                 cells in ascending id, a degenerate triangle once per corner it occupies.
+//   edge_neighbors  GetCellEdgeNeighbors through those links.
 //
 // Stable sorts are LSD radix passes of 8 bits (per-block digit histograms, one scan, a scatter ranked by
 // warp match), only over the bits the largest key needs.
@@ -154,6 +156,26 @@ __global__ void __launch_bounds__(kBlock) k_conn_load(Faces F, int32_t* __restri
 
 __global__ void __launch_bounds__(kBlock) k_copy_i32(const uint32_t* __restrict__ in, int64_t n, int32_t* out) {
   for (int64_t i = gtid(); i < n; i += gstride()) out[i] = (int32_t)in[i];
+}
+
+// GetCellEdgeNeighbors(c, p1, p2) over the links: the cells d != c in p1's links that contain p2, in link
+// order, duplicates included. Returns their number; *first becomes the first of them and *lowest the lowest
+// (both unchanged when there is none).
+__device__ __forceinline__ int64_t edge_neighbors(const int32_t* __restrict__ tri,
+                                                  const unsigned long long* __restrict__ lstart,
+                                                  const int32_t* __restrict__ links, int64_t c, int32_t p1,
+                                                  int32_t p2, int64_t* first, int64_t* lowest) {
+  int64_t num = 0;
+  for (unsigned long long k = lstart[p1]; k < lstart[p1 + 1]; ++k) {
+    const int32_t d = links[k];
+    if (d == c) continue;
+    if (tri[3 * (int64_t)d] == p2 || tri[3 * (int64_t)d + 1] == p2 || tri[3 * (int64_t)d + 2] == p2) {
+      if (num == 0) *first = d;
+      ++num;
+      if (d < *lowest) *lowest = d;
+    }
+  }
+  return num;
 }
 
 // Loads the faces into w.tri and builds w.lstart [V + 1] and w.links [3T] (nt > 0). W also holds status and

@@ -138,16 +138,8 @@ __global__ void __launch_bounds__(kBlock) k_sm_edges(const float* __restrict__ P
     const int64_t c = q / 3;
     const int i = (int)(q - 3 * c);
     const int32_t p1 = tri[q], p2 = tri[3 * c + (i + 1) % 3];
-    int64_t num = 0, lowest = INT64_MAX, nei = -1;
-    for (unsigned long long k = lstart[p1]; k < lstart[p1 + 1]; ++k) {
-      const int32_t d = links[k];
-      if (d == c) continue;
-      if (tri[3 * (int64_t)d] == p2 || tri[3 * (int64_t)d + 1] == p2 || tri[3 * (int64_t)d + 2] == p2) {
-        if (num == 0) nei = d;
-        ++num;
-        if (d < lowest) lowest = d;
-      }
-    }
+    int64_t lowest = INT64_MAX, nei = -1;
+    const int64_t num = edge_neighbors(tri, lstart, links, c, p1, p2, &nei, &lowest);
     uint8_t e = SIMPLE;
     if (num == 0) {
       e = BOUNDARY;

@@ -112,3 +112,30 @@ def smooth_polydata(vertices: np.ndarray, faces: np.ndarray, iterations: int = 2
                                torch.from_numpy(np.ascontiguousarray(faces)).cuda(), iterations, relaxation_factor,
                                feature_angle, edge_angle, feature_edge_smoothing, boundary_smoothing, convergence)
     return r.vertices.cpu().numpy()
+
+
+# polydata_utils.ApplySmoothFilter: the smoother with these settings, then vtkFillHolesFilter at HoleSize 1000
+_APPLY_SMOOTH = dict(feature_angle=80.0, feature_edge_smoothing=False, boundary_smoothing=False)
+_APPLY_SMOOTH_HOLE_SIZE = 1000.0
+
+
+def apply_smooth_filter_device(vertices: torch.Tensor, faces: torch.Tensor, iterations: int,
+                               relaxation_factor: float) -> tuple[torch.Tensor, torch.Tensor]:
+    """ApplySmoothFilter ("Smooth surface") on device tensors: (smoothed vertices, faces with the holes of
+    radius <= 1000 filled, in the input's dtype and form). Synchronises."""
+    from .surface_holes import fill_holes_device
+    s = smooth_polydata_device(vertices, faces, iterations, relaxation_factor, **_APPLY_SMOOTH)
+    return s.vertices, fill_holes_device(s.vertices, faces, _APPLY_SMOOTH_HOLE_SIZE).faces
+
+
+def apply_smooth_filter(vertices: np.ndarray, faces: np.ndarray, iterations: int,
+                        relaxation_factor: float) -> tuple[np.ndarray, np.ndarray]:
+    """ApplySmoothFilter ("Smooth surface") on numpy arrays: (float32 [V,3] vertices, faces)."""
+    if not isinstance(vertices, np.ndarray) or not isinstance(faces, np.ndarray):
+        raise TypeError("smoothing: numpy arrays expected")
+    _check(vertices, faces, iterations)
+    require_cuda()
+    v, f = apply_smooth_filter_device(torch.from_numpy(np.ascontiguousarray(vertices)).cuda(),
+                                      torch.from_numpy(np.ascontiguousarray(faces)).cuda(), iterations,
+                                      relaxation_factor)
+    return v.cpu().numpy(), f.cpu().numpy()
