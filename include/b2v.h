@@ -265,6 +265,40 @@ int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t nx, const ui
 int b2v_count_regions(const void* image, int dtype, int64_t n, uint32_t number_regions, uint32_t* out, void* workspace,
                       void* stream);
 
+/* Labelling of a Z-sharded volume (dist.label): every shard labels its own planes with b2v_label
+ * (local labels 1..n_r); the provisional id of local label l on shard r is P = base_r + l, base_r the
+ * sum of the lower shards' counts. These three stages turn provisional ids into SciPy's numbering of
+ * the whole volume. Ids are int64, labels uint32.
+ * b2v_label_boundary_count / _emit: the boundary between a shard and the next one. lo_plane = the
+ *   lower shard's last plane of local labels (ids 1..n_lo), hi_plane = the upper shard's first plane
+ *   (ids 1..n_hi), both [ny][nx]. Every foreground voxel below is paired with the foreground voxels
+ *   above at the structure's z = +1 offsets (strct_host as for b2v_label); the pairs are reduced to a
+ *   spanning forest in which the root of a set is its smallest id, and one pair (P, P(root)) is made for
+ *   every label on the two planes that is not a root: at most one per distinct label. _count builds the
+ *   forest and reports the pair count (SYNCHRONISES; 0 without building anything when the structure is 1
+ *   wide along z); _emit writes the npairs pairs, int64 [npairs][2], in the order of each label's first
+ *   voxel (lower plane first, raster order), with base_lo = the lower shard's base. Both calls share one
+ *   workspace of b2v_label_boundary_workspace_bytes(ny, nx, n_lo, n_hi) bytes; only the labels on the
+ *   two planes are touched in it. 2 ny nx < 2^31 and n_lo + n_hi < 2^31 - 1.
+ * b2v_label_resolve: the pairs of every boundary, int64 [npairs][2], and ends = their distinct
+ *   endpoints, sorted (int64 [nends]). Union-find over the endpoints, the larger root under the
+ *   smaller; M = the endpoints that are not their set's root. Writes lut[l] = Final(base + l) for
+ *   l in [0, nlocal] (lut[0] = 0), Final(P) = R - |{Q in M : Q < R}| with R = the root of P's set (P
+ *   itself when it is no endpoint): the rank of the component's smallest provisional id among all
+ *   components. *nmerged_host = |M|, so the volume holds sum(n_r) - |M| labels. SYNCHRONISES; an endpoint
+ *   missing from ends is B2V_ERR_ARG. workspace: b2v_label_resolve_workspace_bytes(nends).
+ * b2v_label_relabel: labels[i] = lut[labels[i]] over n labels (values >= nlut are left as they are). */
+int64_t b2v_label_boundary_workspace_bytes(int64_t ny, int64_t nx, int64_t n_lo, int64_t n_hi);
+int b2v_label_boundary_count(const uint32_t* lo_plane, const uint32_t* hi_plane, int64_t ny, int64_t nx,
+                             const uint8_t* strct_host, int64_t odz, int64_t ody, int64_t odx, int64_t n_lo, int64_t n_hi,
+                             void* workspace, void* stream, int64_t* npairs_host);
+int b2v_label_boundary_emit(const uint32_t* lo_plane, const uint32_t* hi_plane, int64_t ny, int64_t nx, int64_t n_lo,
+                            int64_t n_hi, int64_t base_lo, int64_t npairs, int64_t* pairs, void* workspace, void* stream);
+int64_t b2v_label_resolve_workspace_bytes(int64_t nends);
+int b2v_label_resolve(const int64_t* pairs, int64_t npairs, const int64_t* ends, int64_t nends, int64_t base,
+                      int64_t nlocal, uint32_t* lut, void* workspace, void* stream, int64_t* nmerged_host);
+int b2v_label_relabel(uint32_t* labels, int64_t n, const uint32_t* lut, int64_t nlut, void* stream);
+
 /* ---- view-matrix resampling (SURVEY 8f-1) --------------------------------------------
  * invesalius_rs.apply_view_matrix_transform(volume, spacing, M, n, orientation, minterpol, cval,
  * out): __init__.py:84 -> transforms_py.rs:96-148 -> transforms.rs:9-55 -> interpolation.rs.

@@ -68,6 +68,12 @@ PROTOTYPES = {
     "b2v_label_workspace_bytes": (i64, [i64]),
     "b2v_label": (cint, [vp, i64, i64, i64, vp, i64, i64, i64, vp, vp, vp, C.POINTER(i64)]),
     "b2v_count_regions": (cint, [vp, cint, i64, u32, vp, vp, vp]),
+    "b2v_label_boundary_workspace_bytes": (i64, [i64, i64, i64, i64]),
+    "b2v_label_boundary_count": (cint, [vp, vp, i64, i64, vp, i64, i64, i64, i64, i64, vp, vp, C.POINTER(i64)]),
+    "b2v_label_boundary_emit": (cint, [vp, vp, i64, i64, i64, i64, i64, i64, vp, vp, vp]),
+    "b2v_label_resolve_workspace_bytes": (i64, [i64]),
+    "b2v_label_resolve": (cint, [vp, i64, vp, i64, i64, i64, vp, vp, vp, C.POINTER(i64)]),
+    "b2v_label_relabel": (cint, [vp, i64, vp, i64, vp]),
     "b2v_apply_view_matrix_transform": (cint, [vp, cint, i64, i64, i64, vp, vp, i64, cint, cint, dbl, vp, i64, i64, i64, vp,
                                                vp]),
     "b2v_mc_workspace_bytes": (i64, [i64, i64, i64]),

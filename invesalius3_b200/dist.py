@@ -14,7 +14,13 @@ op of the path is sharded the same way (SURVEY.md section 8e):
                        differences), then the sharded MaxIP / LMIP / MIDA of its own planes
   watershed            local convergence with frozen halo planes, boundary planes swapped (costs,
                        then keys + label sets) until no halo plane improves
-  fill holes           per-shard label histogram, one all_reduce, local apply
+  labelling            local labels of the own planes, one all_gather of the counts; the next
+                       shard's first plane of labels sent down (4 x dy x dx bytes); each boundary's
+                       pairs reduced to a spanning forest (one pair per non-root label on the two
+                       planes), the forests all_gathered and resolved alike on every rank, then one
+                       relabel pass: SciPy's numbering of the whole volume, no iteration
+  fill holes           per-shard label histogram, one all_reduce, local apply; fill_holes_auto
+                       labels the unselected voxels with the sharded labelling first
   flood fill           local convergence on slab + one halo plane per inner side, then the
                        reached bits of the two shared planes are swapped with each neighbour
                        (2 x dy x dx/8 bytes) and merged; repeat until no shard gains a bit.
@@ -415,6 +421,47 @@ class DeviceBackend:
     def fh_apply(self, st, max_size):
         self._fh(st, 2, max_size)
         return bool(st["mod"].value)
+
+    # -- labelling (own planes only; labels are int32 tensors holding uint32 ids)
+    def lb_local(self, fg, structure):
+        from . import labeling
+        return labeling.label_device(fg, structure)
+
+    def lb_boundary(self, lo_plane, hi_plane, structure, base_lo, n_lo, n_hi):
+        """int64 [m, 2] spanning-forest pairs (P, P(root)) of the boundary between lo_plane (my last
+        plane) and hi_plane (the next shard's first plane)."""
+        dev, lib = self.dev, self._lib.load()
+        lo_plane, hi_plane = lo_plane.contiguous(), hi_plane.contiguous()
+        ny, nx = lo_plane.shape
+        ws = dev._workspace(lib.b2v_label_boundary_workspace_bytes(ny, nx, int(n_lo), int(n_hi)), lo_plane.device)
+        m = C.c_int64(0)
+        with torch.cuda.device(lo_plane.device):
+            self._lib.call("b2v_label_boundary_count", dev._p(lo_plane), dev._p(hi_plane), ny, nx,
+                           C.c_void_p(structure.ctypes.data), *structure.shape, int(n_lo), int(n_hi), dev._p(ws),
+                           dev._stream(), C.byref(m))
+            pairs = torch.empty((m.value, 2), dtype=torch.int64, device=lo_plane.device)
+            self._lib.call("b2v_label_boundary_emit", dev._p(lo_plane), dev._p(hi_plane), ny, nx, int(n_lo), int(n_hi),
+                           int(base_lo), m.value, dev._p(pairs), dev._p(ws), dev._stream())
+        return pairs
+
+    def lb_resolve(self, pairs, base, nlocal):
+        """(lut, |M|): the int32 (uint32 bits) table [nlocal + 1] of my labels' final ids."""
+        dev, lib = self.dev, self._lib.load()
+        pairs = pairs.contiguous()
+        ends = torch.unique(pairs.reshape(-1))          # sorted: compacts the endpoints
+        lut = torch.empty(int(nlocal) + 1, dtype=torch.int32, device=pairs.device)
+        ws = dev._workspace(lib.b2v_label_resolve_workspace_bytes(ends.numel()), pairs.device)
+        nm = C.c_int64(0)
+        with torch.cuda.device(pairs.device):
+            self._lib.call("b2v_label_resolve", dev._p(pairs), pairs.shape[0], dev._p(ends), ends.numel(), int(base),
+                           int(nlocal), dev._p(lut), dev._p(ws), dev._stream(), C.byref(nm))
+        return lut, int(nm.value)
+
+    def lb_relabel(self, labels, lut):
+        with torch.cuda.device(labels.device):
+            self._lib.call("b2v_label_relabel", self.dev._p(labels), labels.numel(), self.dev._p(lut), lut.numel(),
+                           self.dev._stream())
+        return labels
 
     # -- watershed (extended slab; halo planes frozen)
     def ws_preprocess(self, image_i16, use_ww_wl, wl, ww, global_min=None):
@@ -825,3 +872,72 @@ def fill_holes_automatically(mask_slab, labels_slab, nlabels, max_size, shard: Z
     st = be.fh_hist(mask_slab, labels_slab, nlabels)
     _all_reduce(shard, be.fh_sizes(st), dist.ReduceOp.SUM)
     return be.fh_apply(st, max_size)
+
+
+def label(fg_slab, structure, shard: ZShard, backend=None):
+    """scipy.ndimage.label of the Z-sharded volume: fg_slab is this shard's own planes (uint8 / bool,
+    non-zero = feature, no halo). Returns (labels, total): an int32 tensor holding the uint32 labels of
+    the own planes, numbered as SciPy numbers the whole volume, and the number of labels of the whole
+    volume, identical on every rank.
+
+    Each shard labels its slab (local labels 1..n_r in its raster order); provisional id base_r + l,
+    base_r the lower shards' label count (one all_gather). With a structure 3 wide along z, the next
+    shard sends its first plane of local labels down (4 dy dx bytes) and each boundary reduces its
+    pairs to a spanning forest, one pair per non-root label on the two planes; the forests are
+    all_gathered, every rank resolves them alike (union-find, root = smallest id) and relabels its
+    slab through a table. Final = rank of the component's smallest provisional id, which is the rank
+    of its first voxel in raster order: SciPy's numbering. Four collectives, whatever the volume."""
+    from . import labeling
+    if shard.DZ < shard.world:
+        raise ValueError(f"dist.label: {shard.DZ} planes cannot give each of {shard.world} shards one")
+    if fg_slab.dim() != 3 or fg_slab.shape[0] != shard.z1 - shard.z0:
+        raise ValueError(f"dist.label: expected this shard's {shard.z1 - shard.z0} own planes")
+    st = labeling._structure(structure, 3)
+    be = _backend(backend)
+    labels, n = be.lb_local(fg_slab, st)
+    dev = labels.device
+    counts = _all_gather_rows(shard, torch.tensor([[int(n)]], dtype=torch.int64, device=dev), [1] * shard.world)
+    counts = [int(c) for c in counts.reshape(-1).cpu()]
+    base = sum(counts[:shard.rank])
+    pairs = torch.zeros((0, 2), dtype=torch.int64, device=dev)
+    if st.shape[0] == 3 and st[2].any() and shard.world > 1:
+        ops, hi_plane = [], None
+        if shard.has_lo:
+            ops.append(dist.P2POp(dist.isend, _stage(shard, labels[0].contiguous()), shard.rank - 1, group=shard.group))
+        if shard.has_hi:
+            hi_plane = _stage(shard, torch.empty_like(labels[0]))
+            ops.append(dist.P2POp(dist.irecv, hi_plane, shard.rank + 1, group=shard.group))
+        for req in dist.batch_isend_irecv(ops):
+            req.wait()
+        if shard.has_hi:
+            pairs = be.lb_boundary(labels[-1], hi_plane.to(dev), st, base, counts[shard.rank], counts[shard.rank + 1])
+        sizes = _all_gather_rows(shard, torch.tensor([[pairs.shape[0]]], dtype=torch.int64, device=dev), [1] * shard.world)
+        sizes = [int(c) for c in sizes.reshape(-1).cpu()]
+        if sum(sizes):      # padded here: a shard may have no pairs to send
+            m = max(sizes)
+            mine = torch.zeros((m, 2), dtype=torch.int64, device=dev)
+            mine[:pairs.shape[0]] = pairs
+            every = _all_gather_rows(shard, mine, [m] * shard.world)
+            pairs = torch.cat([every[r * m: r * m + c] for r, c in enumerate(sizes)])
+    lut, merged = be.lb_resolve(pairs, base, n)
+    total = sum(counts) - merged
+    if total >= 2 ** 32:
+        raise ValueError("dist.label: more than 2^32 - 1 labels do not fit uint32")
+    if n and (base or pairs.shape[0]):
+        be.lb_relabel(labels, lut)
+    return labels, total
+
+
+def fill_holes_auto(mask_slab, conn, size, shard: ZShard, backend=None) -> bool:
+    """labeling.fill_holes_auto (Mask.fill_holes_auto, mask.py:523-537) on a Z-sharded mask body:
+    mask_slab is this shard's own planes (uint8), rewritten in place. The unselected voxels are labelled
+    with dist.label, then fill_holes_automatically fills the components of at most `size` voxels with
+    254. No label image of the whole mask exists anywhere. Returns the same bool on every rank."""
+    from scipy.ndimage import generate_binary_structure
+    if mask_slab.dtype != torch.uint8 or mask_slab.dim() != 3:
+        raise TypeError("Invalid mask type")
+    st = generate_binary_structure(3, {6: 1, 18: 2, 26: 3}[conn])
+    labels, n = label((~(mask_slab > 127)).to(torch.uint8), st, shard, backend=backend)
+    if n == 0:
+        return False
+    return fill_holes_automatically(mask_slab, labels, n, int(size), shard, backend=backend)
