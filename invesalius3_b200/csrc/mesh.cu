@@ -4,19 +4,25 @@
 // normals [M][3]. The reference's stages, each a kernel over the vertices:
 //   vertex -> faces   (build_map_vface :89-101): CSR from the caller's stable ordering of the 4 M face
 //                     entries — EVERY column is taken as a vertex id, the leading 3 included, as the
-//                     reference does (vertex 3 collects every face);
+//                     reference does (vertex 3 collects every face). The reference only looks the map up
+//                     for ids in [0, V), so a leading entry outside that range is ignored (a mesh of at
+//                     most 3 vertices is valid); an entry of columns 1..3 outside it is an error;
 //   adjacency         (build_vertex_connectivity :103-123): neighbours in first-appearance order over the
 //                     faces — the order fixes the float64 summation order of the smoother;
 //   staircase seeds   (find_staircase_artifacts :125-189): the reference's max / min tracking with its
-//                     `else if`, kept as it is (after a vertex's first face min is still f64::MAX, so
-//                     every vertex that has a face becomes a seed);
+//                     `else if`, kept as it is. After a vertex's first face min is still f64::MAX, so
+//                     every vertex that has a face becomes a seed for any finite T (none for T = NaN);
+//                     for T = +inf a vertex is a seed exactly when its first face has a NaN normal
+//                     (|f64::MIN - f64::MAX| overflows to inf);
 //   weights           (propagate_weights :202-295): frontier rounds; a round is resolved by atomic minimum
 //                     on the squared distance, then the seed of the winner (smallest seed on ties) — the
-//                     reference resolves a round by compare-and-swap in whatever order its threads run;
+//                     reference resolves a round by compare-and-swap in whatever order its threads run.
+//                     With every seed at distance 0 the first round claims nothing: the later rounds
+//                     run only for T = +inf with NaN normals;
 //   Taubin            (taubin_smooth :345-395): lambda 0.5, mu -0.53; D in float64 in adjacency order,
 //                     updates cast to float32 and added in float32.
-// Bit-exact against the sequential CPU restatement of the tests whenever the rounds of the weight
-// propagation have no ties between different seeds (always, with the reference's seeding).
+// Bit-exact against the sequential CPU checker whenever no vertex receives offers from two seeds, and against
+// the round-by-round schedule of the NumPy restatement in tests/ca_smoothing_model.py.
 #include "b2v_common.cuh"
 
 namespace {
@@ -58,13 +64,14 @@ MeshWs carve(void* base, long long nv, long long nf) {
   return w;
 }
 
-// entries sorted by vertex id (stable): segment bounds per vertex; an entry outside [0, V) is an error
+// entries sorted by vertex id (stable): segment bounds per vertex. A leading-column entry outside [0, V) is
+// skipped (the reference never looks it up); an entry of columns 1..3 outside [0, V) is an error
 __global__ void __launch_bounds__(256) k_mesh_segments(const long long* __restrict__ faces, const long long* __restrict__ order,
                                                        long long ne, long long nv, long long* first, long long* last, int* status) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < ne; e += stride) {
-    const long long key = faces[order[e]];
-    if (key < 0 || key >= nv) { *status = 1; continue; }
+    const long long ent = order[e], key = faces[ent];
+    if (key < 0 || key >= nv) { if (ent & 3) *status = 1; continue; }
     if (e == 0 || faces[order[e - 1]] != key) first[key] = e;
     if (e == ne - 1 || faces[order[e + 1]] != key) last[key] = e + 1;
   }
@@ -108,15 +115,21 @@ __device__ __forceinline__ int for_each_neighbour(const long long* __restrict__ 
   return k;
 }
 
-// faces around a vertex (columns 1..3 only): the host refuses meshes with more than kMaxRing
+// distinct faces around a vertex (columns 1..3 only), counted as for_each_neighbour counts them: the host
+// refuses meshes with more than kMaxRing
 __global__ void __launch_bounds__(256) k_mesh_ring_check(const long long* __restrict__ order, long long nv,
                                                          const long long* __restrict__ first, const long long* __restrict__ last,
                                                          int* status) {
   const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nv || first[v] < 0) return;
   if (last[v] - first[v] <= kMaxRing) return;     // cannot exceed it
-  long long n = 0;
-  for (long long e = first[v]; e < last[v]; ++e) n += (order[e] & 3) != 0;
+  long long n = 0, prev_fb = -1;
+  for (long long e = first[v]; e < last[v]; ++e) {
+    const long long ent = order[e];
+    if ((ent & 3) == 0 || (ent & ~3ll) == prev_fb) continue;    // v twice in one face: one face
+    prev_fb = ent & ~3ll;
+    ++n;
+  }
   if (n > kMaxRing) *status = 2;
 }
 
@@ -321,7 +334,7 @@ extern "C" int b2v_ca_smoothing(float* vertices, int64_t nverts, const int64_t* 
   int st = 0;
   B2V_CUDA(cudaMemcpyAsync(&st, w.status, 4, cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));
-  B2V_REQUIRE(st == 0, B2V_ERR_RANGE, "ca_smoothing: a face entry lies outside the vertex array (the reference panics here)");
+  B2V_REQUIRE(st == 0, B2V_ERR_RANGE, "ca_smoothing: a face entry (columns 1..3) lies outside the vertex array (the reference panics here)");
   k_mesh_ring_check<<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>((const long long*)order, nv, w.first, w.last, w.status);
   if ((rc = b2v_check_launch("k_mesh_ring_check"))) return rc;
   B2V_CUDA(cudaMemcpyAsync(&st, w.status, 4, cudaMemcpyDeviceToHost, s));

@@ -17,8 +17,19 @@ from . import device as dev
 from .device import _p, _stream, _workspace
 
 
+def _n_iters(n_iters) -> int:
+    """The reference's `n_iters: u32`: PyO3 raises OverflowError outside [0, 2**32)."""
+    n = int(n_iters)
+    if n < 0:
+        raise OverflowError("can't convert negative int to unsigned")
+    if n > 0xFFFFFFFF:
+        raise OverflowError("out of range integral type conversion attempted")
+    return n
+
+
 def smooth_device(verts: torch.Tensor, faces4: torch.Tensor, normals: torch.Tensor, T, tmax, bmin, n_iters) -> None:
     """float32 [V,3] / int64 [M,4] / float32 [M,3] device tensors; verts is modified in place."""
+    n_iters = _n_iters(n_iters)
     if verts.dtype != torch.float32 or faces4.dtype != torch.int64 or normals.dtype != torch.float32:
         raise TypeError("ca_smoothing: float32 vertices, int64 faces, float32 normals")
     if faces4.dim() != 2 or faces4.shape[1] != 4 or normals.shape != (faces4.shape[0], 3) or verts.dim() != 2 or verts.shape[1] != 3:
@@ -33,7 +44,7 @@ def smooth_device(verts: torch.Tensor, faces4: torch.Tensor, normals: torch.Tens
     ws = _workspace(_lib.load().b2v_ca_smoothing_workspace_bytes(nv, nf), verts.device)
     with torch.cuda.device(verts.device):
         _lib.call("b2v_ca_smoothing", _p(verts), nv, _p(faces4), nf, _p(normals), _p(order), float(T), float(tmax), float(bmin),
-                  int(n_iters), _p(ws), _stream())
+                  n_iters, _p(ws), _stream())
 
 
 def context_aware_smoothing(vertices, faces, normals, T, tmax, bmin, n_iters) -> None:
@@ -45,9 +56,7 @@ def context_aware_smoothing(vertices, faces, normals, T, tmax, bmin, n_iters) ->
         raise TypeError("Invalid normals type")
     if not vertices.flags.writeable:
         raise ValueError("vertices is read-only")
-    n_iters = int(n_iters)
-    if n_iters < 0:
-        raise OverflowError("can't convert negative int to unsigned")
+    n_iters = _n_iters(n_iters)
     v = torch.from_numpy(np.ascontiguousarray(vertices)).cuda()
     f = torch.from_numpy(np.ascontiguousarray(faces).astype(np.int64)).cuda()
     n = torch.from_numpy(np.ascontiguousarray(normals, dtype=np.float32)).cuda()   # as_(): float64 normals enter the float64 test exactly

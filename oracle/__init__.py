@@ -258,7 +258,9 @@ def _mida_f64_f64(image, axis, wl, ww, out):
 # --------------------------------------------------------------------------- mesh smoothing
 def ca_smoothing(vertices, faces, normals, T, tmax, bmin, n_iters, return_weights=False):
     """invesalius_rs.context_aware_smoothing (mesh_py.rs -> mesh.rs:27-395) on float32 vertices [V,3]
-    (modified in place), int64 faces [M,4] (leading 3) and float32 face normals [M,3]. PARITY UNPINNED."""
+    (modified in place), int64 faces [M,4] (leading 3) and float32 face normals [M,3]. Checked by the NumPy
+    restatement of tests/ca_smoothing_model.py; parity with the crate unpinned. IndexError: an entry of
+    columns 1..3 outside the vertex array (the crate panics); the leading column may hold any value."""
     if vertices.dtype != np.float32 or faces.dtype != np.int64 or normals.dtype != np.float32:
         raise TypeError("ca_smoothing checker: float32 vertices, int64 faces, float32 normals")
     assert vertices.flags.c_contiguous and faces.flags.c_contiguous and normals.flags.c_contiguous and faces.shape[1] == 4
@@ -266,7 +268,7 @@ def ca_smoothing(vertices, faces, normals, T, tmax, bmin, n_iters, return_weight
     rc = lib().orc_ca_smoothing(_ptr(vertices), C.c_int64(len(vertices)), _ptr(faces), C.c_int64(len(faces)), _ptr(normals),
                                 C.c_double(T), C.c_double(tmax), C.c_double(bmin), C.c_uint32(int(n_iters)), _ptr(w))
     if rc:
-        raise IndexError("face entry outside the vertex array")
+        raise IndexError("face entry (columns 1..3) outside the vertex array")
     return w if return_weights else None
 
 

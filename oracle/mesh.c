@@ -3,16 +3,20 @@
  * context_aware_smoothing: invesalius_rs/src/mesh.rs:27-395 (float32 vertices, int64 faces [M][4] with
  * the leading 3, float32 face normals), restated sequentially in the reference's iteration order:
  *   build_map_vface          :89-101  every column of a face row is taken as a vertex id, the leading 3
- *                                      included (so vertex 3 collects every face) — kept as it is
+ *                                      included (so vertex 3 collects every face) — kept as it is; the
+ *                                      map is only looked up for ids in [0, nv), so a leading entry
+ *                                      outside that range is ignored
  *   build_vertex_connectivity:103-123 neighbours in first-appearance order over the faces
  *   find_staircase_artifacts :125-189 the max / min tracking with its `else if` (after the first face min
- *                                      is still f64::MAX, so |max - min| >= t: every vertex that has a
- *                                      face is returned) — kept as it is
+ *                                      is still f64::MAX, so |max - min| >= t: for finite t every vertex
+ *                                      that has a face is returned; for t = inf, those whose first face
+ *                                      has a NaN normal) — kept as it is
  *   propagate_weights        :202-295 frontier by frontier; the reference runs a frontier in parallel
  *                                      with compare-and-swap (its result can depend on thread timing);
  *                                      here the frontier is walked in order, one valid execution
  *   taubin_smooth            :345-395 lambda 0.5, mu -0.53, float64 sums in adjacency order, float32 updates
- * The reference has no test for this function: PARITY UNPINNED. */
+ * The reference has no test for this function: PARITY UNPINNED. tests/ca_smoothing_model.py, written from
+ * mesh.rs independently of this file, pins it bit for bit. */
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -34,21 +38,22 @@ static void calc_d(const float* v, const Csr* adj, int64_t i, double d[3]) {
   if (n > 0) { d[0] /= (double)n; d[1] /= (double)n; d[2] /= (double)n; }
 }
 
-/* weights_out (optional): float64 [nv]. Returns 0, or 1 on a face entry outside [0, nv). */
+/* weights_out (optional): float64 [nv]. Returns 0, or 1 on an entry of columns 1..3 outside [0, nv). */
 int orc_ca_smoothing(float* vertices, int64_t nv, const int64_t* faces, int64_t nf, const float* normals, double t,
                      double tmax, double bmin, uint32_t n_iters, double* weights_out) {
   /* map_vface as CSR, entries in (face, column) order */
   int64_t* cnt = (int64_t*)calloc((size_t)nv + 1, 8);
   for (int64_t e = 0; e < 4 * nf; ++e) {
-    if (faces[e] < 0 || faces[e] >= nv) { free(cnt); return 1; }
-    ++cnt[faces[e] + 1];
+    if (faces[e] >= 0 && faces[e] < nv) ++cnt[faces[e] + 1];
+    else if (e % 4 != 0) { free(cnt); return 1; }
   }
   for (int64_t i = 0; i < nv; ++i) cnt[i + 1] += cnt[i];
   int64_t* vf = (int64_t*)malloc((size_t)(4 * nf + 1) * 8);
   int64_t* fill = (int64_t*)malloc((size_t)nv * 8);
   memcpy(fill, cnt, (size_t)nv * 8);
   for (int64_t f = 0; f < nf; ++f)
-    for (int c = 0; c < 4; ++c) vf[fill[faces[4 * f + c]]++] = f;
+    for (int c = 0; c < 4; ++c)
+      if (faces[4 * f + c] >= 0 && faces[4 * f + c] < nv) vf[fill[faces[4 * f + c]]++] = f;
   /* vertex connectivity */
   Csr adj;
   int64_t cap = 16 * nv + 16, used = 0;
