@@ -641,7 +641,7 @@ int b2v_ws_flood(const uint16_t* img, const int16_t* markers, int64_t nz, int64_
  * that is never relaxed locally; b2v_ws_plane reads a plane (merge = 0) or merges a neighbour's
  * values into one (merge = 1: minimum of the costs / of the keys, join of the label sets; tiles
  * next to a voxel that changed are queued for the next *_CONVERGE; *changed_host = 1 if any did).
- * what = 0: uint32 costs (phase 1); what = 1: uint64 keys followed by uint16 label sets (phase 2);
+ * what = 0: uint32 costs (phase 1); what = 1: uint64 keys followed by uint32 label sets (phase 2);
  * plane buffers are device memory of b2v_ws_plane_bytes(ny, nx, what) bytes.
  * stages (bit mask, executed in this order): 1 INIT, 2 COST_CONVERGE, 4 LABEL_BEGIN (admissible
  * predecessors from the final costs), 8 LABEL_CONVERGE, 16 FINISH (labels + ambiguous mask out).
@@ -656,7 +656,9 @@ int b2v_ws_plane(int merge, int what, int64_t nz, int64_t ny, int64_t nx, int mo
                  int64_t z, void* plane, void* workspace, void* stream, int* changed_host);
 int b2v_ws_shift_i16_with(const int16_t* img, int64_t n, const float* minmax_dev, uint16_t* out, void* stream);
 /* diagnostics of the persistent engine: [0..2] phase-1 tile visits / sweep sets / visits that
- * changed something, [4..6] the same for phase 2; reset != 0 clears them */
+ * changed something, [4..6] the same for phase 2, [3] visits that re-queued their own tile (not
+ * settled within the sweep-set cap, either phase), [7] phase-2 runs on 32-bit keys stopped by the
+ * 24-bit hop limit (and re-run on 64-bit keys); reset != 0 clears them */
 int b2v_ws_stats(int* out8, int reset);
 
 /* ---- Z-sharded volumes (one shard per GPU; invesalius3_b200/dist.py drives these) ---------

@@ -147,9 +147,11 @@ constexpr int kMaxRounds = 1 << 16;
 constexpr uint32_t kInfC = 0xffffffffu;
 constexpr unsigned long long kInfK = ~0ull;
 // label SET of a voxel (phase 2): which labels can reach it along cost-optimal edges, whatever
-// the reference's queue order. code = label + 32768; kSetEmpty = nothing yet; kSetMulti = two
-// different labels (the reference's answer there is an artefact of its queue order).
-constexpr uint16_t kSetEmpty = 32768, kSetMulti = 0;
+// the reference's queue order. uint32: code = label + 32768 for one label (every int16 label is a
+// legal code); kSetEmpty = nothing yet (the code of label 0, which no marker carries); kSetMulti =
+// two different labels (the reference's answer there is an artefact of its queue order), above the
+// 16-bit code range.
+constexpr uint32_t kSetEmpty = 32768, kSetMulti = 0x10000;
 
 struct Grid {
   int64_t nz, ny, nx;
@@ -165,7 +167,7 @@ Grid make_grid(int64_t nz, int64_t ny, int64_t nx) {
 struct WsWs {
   uint32_t* cost;
   unsigned long long* key;
-  uint16_t* lset;
+  uint32_t* lset;
   uint8_t* active[2];
   int* flags;
   int64_t bytes;
@@ -177,7 +179,7 @@ WsWs carve(void* base, const Grid& g) {
   int64_t off = 0;
   w.key = (unsigned long long*)(p + off); off += align256(n * 8);
   w.cost = (uint32_t*)(p + off); off += align256(n * 4);
-  w.lset = (uint16_t*)(p + off); off += align256(n * 2);
+  w.lset = (uint32_t*)(p + off); off += align256(n * 4);
   w.active[0] = (uint8_t*)(p + off); off += align256(nt);
   w.active[1] = (uint8_t*)(p + off); off += align256(nt);
   w.flags = (int*)(p + off); off += align256((int64_t)(kMaxRounds + 2) * 4);
@@ -189,7 +191,7 @@ WsWs carve(void* base, const Grid& g) {
 // tile holding a marker is active in round 0.
 __global__ void __launch_bounds__(256) k_ws_init(const uint16_t* __restrict__ img, const int16_t* __restrict__ markers,
                                                  Grid g, int mode, uint32_t* __restrict__ cost,
-                                                 unsigned long long* __restrict__ key, uint16_t* __restrict__ lset,
+                                                 unsigned long long* __restrict__ key, uint32_t* __restrict__ lset,
                                                  uint8_t* active, int* flags) {
   const int64_t n = g.nz * g.ny * g.nx;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -198,7 +200,7 @@ __global__ void __launch_bounds__(256) k_ws_init(const uint16_t* __restrict__ im
     if (m != 0) {
       cost[i] = mode == 0 ? 0u : (uint32_t)img[i];
       key[i] = (unsigned long long)(uint32_t)(m + 32768);
-      lset[i] = (uint16_t)(m + 32768);
+      lset[i] = (uint32_t)(m + 32768);
       int64_t x = i % g.nx, r = i / g.nx, y = r % g.ny, z = r / g.ny;
       active[((int)(z / kT) * g.nty + (int)(y / kT)) * g.ntx + (int)(x / kT)] = 1;
       flags[0] = 1;
@@ -220,7 +222,7 @@ __global__ void k_ws_activate_all(uint8_t* active, int64_t ntiles, int* flags, i
 // MODE 0: edge weight |I(v) - I(p)|; MODE 1: weight I(p).
 template <int PHASE, int MODE>
 __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restrict__ img, uint32_t* cost,
-                                                       unsigned long long* key, uint16_t* lset, Grid g, uint32_t sb,
+                                                       unsigned long long* key, uint32_t* lset, Grid g, uint32_t sb,
                                                        uint8_t* active_cur, uint8_t* active_next, int* flags,
                                                        int round) {
   if (flags[round] == 0) return;
@@ -228,9 +230,9 @@ __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restric
   if (!__syncthreads_or(active_cur[tile] != 0)) return;
   extern __shared__ unsigned char smem_raw[];
   unsigned long long* sK = (unsigned long long*)smem_raw;                    // PHASE 2 only
-  uint32_t* sC = (uint32_t*)(smem_raw + (PHASE == 2 ? kCells * 8 : 0));
+  uint32_t* sA = (uint32_t*)(smem_raw + kCells * 8);                         // PHASE 2 only
+  uint32_t* sC = (uint32_t*)(smem_raw + (PHASE == 2 ? kCells * 12 : 0));
   uint16_t* sI = (uint16_t*)((unsigned char*)sC + kCells * 4);
-  uint16_t* sA = sI + kCells;                                                 // PHASE 2 only
   __shared__ int s_faces;
   const int tid = threadIdx.x;
   const int tx = tile % g.ntx, ty = (tile / g.ntx) % g.nty, tz = tile / (g.ntx * g.nty);
@@ -244,7 +246,8 @@ __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restric
     int64_t z = z0 + hz - 1, y = y0 + hy - 1, x = x0 + hx - 1;
     uint32_t c = kInfC;
     unsigned long long k = kInfK;
-    uint16_t v = 0, a = kSetEmpty;
+    uint16_t v = 0;
+    uint32_t a = kSetEmpty;
     // MODE 0 reproduces scipy.ndimage.watershed_ift's neighbourhood: the volume is walked as
     // a flat array, a neighbour is any flat index + structure offset inside [0, N), so rows
     // and planes wrap into each other at the volume faces (verified against SciPy 1.18.1).
@@ -306,8 +309,8 @@ __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restric
         if ((kk >> 32) == 0) continue;  // a marker keeps its label
         const uint32_t c = sC[h];
         if (c == kInfC) continue;
-        const uint16_t a0 = sA[h];
-        uint16_t a1 = a0;
+        const uint32_t a0 = sA[h];
+        uint32_t a1 = a0;
         // MODE 1 (label at push time): the voxel inherits from the neighbour that is flooded
         // first, i.e. one with the smallest cost among ALL its neighbours.
         uint32_t cmin = kInfC;
@@ -344,8 +347,8 @@ __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restric
               unsigned long long cand = kv + (1ull << 32);
               best = cand < best ? cand : best;
               // join of the label sets of every admissible predecessor
-              const uint16_t av = sA[v];
-              if (av != kSetEmpty) a1 = (a1 == kSetEmpty) ? av : ((a1 == av && av != kSetMulti) ? a1 : kSetMulti);
+              const uint32_t av = sA[v];
+              if (av != kSetEmpty) a1 = (a1 == kSetEmpty) ? av : (a1 == av ? a1 : kSetMulti);
             }
         if (best < kk || a1 != a0) {
           sK[h] = best;
@@ -425,7 +428,7 @@ __global__ void __launch_bounds__(kThreads) k_ws_round(const uint16_t* __restric
 }
 
 __global__ void __launch_bounds__(256) k_ws_labels(const unsigned long long* __restrict__ key,
-                                                   const uint16_t* __restrict__ lset, int64_t n,
+                                                   const uint32_t* __restrict__ lset, int64_t n,
                                                    int16_t* __restrict__ labels, uint8_t* __restrict__ ambiguous) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -438,7 +441,7 @@ __global__ void __launch_bounds__(256) k_ws_labels(const unsigned long long* __r
 template <int PHASE, int MODE>
 int run_phase(const uint16_t* img, const WsWs& w, const Grid& g, uint32_t sb, cudaStream_t s, int* round_io) {
   const int ntiles = g.ntz * g.nty * g.ntx;
-  const size_t smem = (size_t)kCells * (PHASE == 2 ? 16 : 6);
+  const size_t smem = (size_t)kCells * (PHASE == 2 ? 18 : 6);
   auto kern = k_ws_round<PHASE, MODE>;
   B2V_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int r = *round_io, batch = 4, rc;

@@ -35,7 +35,10 @@ constexpr int kThreads = 256;
 constexpr int kMaxSets = 8;            // sweep sets per visit before the tile re-queues itself
 constexpr uint32_t kInfC = 0xffffffffu;
 constexpr unsigned long long kInfK = ~0ull;
-constexpr uint16_t kSetEmpty = 32768, kSetMulti = 0;
+// label SET of a voxel (watershed.cu): uint32, code = label + 32768 for one label, kSetEmpty = nothing
+// yet (the code of label 0, which no marker carries), kSetMulti = two different labels. Every int16
+// label is a legal code, so "two labels" lives above the 16-bit code range (DESIGN.md section 6).
+constexpr uint32_t kSetEmpty = 32768, kSetMulti = 0x10000;
 // phase-2 key: hops above the label. 64 bits hold any label (uint16 code) and any hop count; when
 // the markers carry at most 256 distinct labels the key is hops << 8 | rank of the label (32 bits):
 // half the chain instructions, shared memory and traffic. kKeyFull32: keys at or above it mean the
@@ -64,14 +67,15 @@ struct FGrid {
 struct Lists {
   uint32_t* bm;   // [3][nbw] tile bitmaps
   int* list;      // [3][ntiles]
-  int* cnt;       // [3] + [3] spare; cnt[4] = error, cnt[5] = rounds, cnt[6] = plane-merge changed flag
+  int* cnt;       // [3] + [3] spare; cnt[4] = error, cnt[5] = rounds, cnt[6] = plane-merge changed flag,
+                  // cnt[8 + (r & 1)] = a 32-bit key of round r reached kKeyFull32
   int nbw;
 };
 
 struct FastWs {
   uint32_t* cost;
   unsigned long long* key;
-  uint16_t* lset;
+  uint32_t* lset;
   uint8_t* adm;
   uint32_t* key32;      // phase-2 keys when the markers carry <= 256 distinct labels
   uint32_t* present;    // [2048] which label codes occur among the markers (bitmap over uint16)
@@ -107,7 +111,7 @@ FastWs fcarve(void* base, int64_t nz, int64_t ny, int64_t nx) {
   int64_t off = 0;
   w.key = (unsigned long long*)(p + off); off += align256(n * 8);
   w.cost = (uint32_t*)(p + off); off += align256(n * 4);
-  w.lset = (uint16_t*)(p + off); off += align256(n * 2);
+  w.lset = (uint32_t*)(p + off); off += align256(n * 4);
   w.adm = (uint8_t*)(p + off); off += align256(n);
   w.key32 = (uint32_t*)(p + off); off += align256(n * 4);
   w.present = (uint32_t*)(p + off); off += 2048 * 4;
@@ -146,7 +150,7 @@ __device__ __forceinline__ long long flat_or_invalid(const FGrid& g, int z, int 
 // ---- init -------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_wsf_init(const uint16_t* __restrict__ img, const int16_t* __restrict__ markers,
                                                   FGrid g, uint32_t* __restrict__ cost,
-                                                  unsigned long long* __restrict__ key, uint16_t* __restrict__ lset,
+                                                  unsigned long long* __restrict__ key, uint32_t* __restrict__ lset,
                                                   Lists L, int* init_list, int* init_cnt, uint32_t* present) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += stride) {
@@ -156,7 +160,7 @@ __global__ void __launch_bounds__(256) k_wsf_init(const uint16_t* __restrict__ i
       if (!((present[code >> 5] >> (code & 31)) & 1u)) atomicOr(&present[code >> 5], 1u << (code & 31));
       cost[i] = g.mode == 0 ? 0u : (uint32_t)img[i];
       key[i] = (unsigned long long)(uint32_t)(m + 32768);
-      lset[i] = (uint16_t)(m + 32768);
+      lset[i] = code;
       const int x = (int)(i % g.nx);
       const long long r = i / g.nx;
       const int y = (int)(r % g.ny), z = (int)(r / g.ny);
@@ -234,7 +238,7 @@ __global__ void __launch_bounds__(256) k_wsf_key32_init(const unsigned long long
   }
 }
 
-__global__ void __launch_bounds__(256) k_wsf_labels32(const uint32_t* __restrict__ key32, const uint16_t* __restrict__ lset,
+__global__ void __launch_bounds__(256) k_wsf_labels32(const uint32_t* __restrict__ key32, const uint32_t* __restrict__ lset,
                                                       const uint32_t* __restrict__ inv, long long n,
                                                       int16_t* __restrict__ labels, uint8_t* __restrict__ ambiguous) {
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -291,7 +295,10 @@ __global__ void __launch_bounds__(256) k_wsf_adm(const uint16_t* __restrict__ im
 }
 
 // ---- tile visits ---------------------------------------------------------------------------------
-__device__ int g_stats[8];   // diagnostics: phase 1 visits / sweep sets / visits that changed, [4..6] phase 2
+// diagnostics: [0..2] phase 1 visits / sweep sets / visits that changed, [4..6] the same for phase 2,
+// [3] visits that re-queued their own tile (not settled within kMaxSets sweep sets, either phase),
+// [7] phase-2 runs on 32-bit keys stopped for the 64-bit re-run
+__device__ int g_stats[8];
 
 struct TileGeom {
   int tz, ty, tx, z0, y0, x0;
@@ -411,12 +418,12 @@ __device__ __forceinline__ void line_full_cost(uint32_t* sC, const uint16_t* sI,
   last = n[kT] != c[kT];
 }
 
-__device__ __forceinline__ uint16_t set_join(uint16_t a, uint16_t b) {   // b != empty
-  return a == kSetEmpty ? b : ((a == b && b != kSetMulti) ? a : kSetMulti);
+__device__ __forceinline__ uint32_t set_join(uint32_t a, uint32_t b) {   // b != empty
+  return a == kSetEmpty ? b : (a == b ? a : kSetMulti);
 }
 
 template <typename K, bool WITH_SET, int S>
-__device__ __forceinline__ void line_full_label(K* sK, uint16_t* sA, const uint8_t* sD, int base,
+__device__ __forceinline__ void line_full_label(K* sK, uint32_t* sA, const uint8_t* sD, int base,
                                                 uint32_t from_lo, uint32_t from_hi, bool& ch, bool& first, bool& last) {
   K k[kT + 2];
   uint32_t av[kT + 2], d[kT + 2];
@@ -436,7 +443,7 @@ __device__ __forceinline__ void line_full_label(K* sK, uint16_t* sA, const uint8
     k[j] = better ? cand : k[j];
     uint32_t ch1 = better ? 1u : 0u;
     if (WITH_SET) {
-      const uint32_t j1 = set_join((uint16_t)av[j], (uint16_t)av[j - 1]);
+      const uint32_t j1 = set_join(av[j], av[j - 1]);
       const bool grow = ok && av[j - 1] != kSetEmpty && j1 != av[j];
       av[j] = grow ? j1 : av[j];
       ch1 |= grow ? 1u : 0u;
@@ -451,7 +458,7 @@ __device__ __forceinline__ void line_full_label(K* sK, uint16_t* sA, const uint8
     k[j] = better ? cand : k[j];
     uint32_t ch1 = better ? 1u : 0u;
     if (WITH_SET) {
-      const uint32_t j1 = set_join((uint16_t)av[j], (uint16_t)av[j + 1]);
+      const uint32_t j1 = set_join(av[j], av[j + 1]);
       const bool grow = ok && av[j + 1] != kSetEmpty && j1 != av[j];
       av[j] = grow ? j1 : av[j];
       ch1 |= grow ? 1u : 0u;
@@ -462,7 +469,7 @@ __device__ __forceinline__ void line_full_label(K* sK, uint16_t* sA, const uint8
   for (int j = 1; j <= kT; ++j)
     if ((m >> j) & 1u) {
       sK[base + (j - 1) * S] = k[j];
-      if (WITH_SET) sA[base + (j - 1) * S] = (uint16_t)av[j];
+      if (WITH_SET) sA[base + (j - 1) * S] = av[j];
     }
   ch = m != 0;
   first = (m >> 1) & 1u;
@@ -639,8 +646,8 @@ __device__ int visit_cost(const uint16_t* __restrict__ img, uint32_t* cost, cons
 
 // PHASE 2: keys (hops << 32 | label) and label sets along admissible edges
 template <typename K, bool WITH_SET>
-__device__ int visit_label(const uint8_t* __restrict__ adm, K* key, uint16_t* lset, const FGrid& g,
-                           const TileGeom& t, K* sK, uint16_t* sA, uint8_t* sD, int* s_faces, int* err) {
+__device__ int visit_label(const uint8_t* __restrict__ adm, K* key, uint32_t* lset, const FGrid& g,
+                           const TileGeom& t, K* sK, uint32_t* sA, uint8_t* sD, int* s_faces, int* err) {
   constexpr bool K64 = sizeof(K) == 8;
   constexpr int KV = K64 ? 8 : 4;     // 128-bit vectors per row of 16 keys
   const int tid = threadIdx.x;
@@ -649,18 +656,18 @@ __device__ int visit_label(const uint8_t* __restrict__ adm, K* key, uint16_t* ls
   if (full) {
     const int a = tid & 15, b = tid >> 4;
     const long long p0 = ((long long)(t.z0 + b) * g.ny + (t.y0 + a)) * g.nx + t.x0;
-    uint4 k4[KV], a4[2], d4;
+    uint4 k4[KV], a4[4], d4;
 #pragma unroll
     for (int k = 0; k < KV; ++k) k4[k] = __ldcg((const uint4*)(key + p0) + k);
     if (WITH_SET) {
 #pragma unroll
-      for (int k = 0; k < 2; ++k) a4[k] = __ldcg((const uint4*)(lset + p0) + k);
+      for (int k = 0; k < 4; ++k) a4[k] = __ldcg((const uint4*)(lset + p0) + k);
     }
     d4 = __ldg((const uint4*)(adm + p0));
     long long hp[6];
     int hc[6];
     K hk[6];
-    uint16_t hs[6];
+    uint32_t hs[6];
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
       hp[k] = halo_cell(g, t, k, a, b, &hc[k]);
@@ -668,7 +675,8 @@ __device__ int visit_label(const uint8_t* __restrict__ adm, K* key, uint16_t* ls
       if (hp[k] >= 0) { hk[k] = __ldcg(&key[hp[k]]); if (WITH_SET) hs[k] = __ldcg(&lset[hp[k]]); }
     }
     const int r0 = cell_index(b + 1, a + 1, 1);
-    const uint32_t aa[8] = {a4[0].x, a4[0].y, a4[0].z, a4[0].w, a4[1].x, a4[1].y, a4[1].z, a4[1].w};
+    const uint32_t aa[16] = {a4[0].x, a4[0].y, a4[0].z, a4[0].w, a4[1].x, a4[1].y, a4[1].z, a4[1].w,
+                             a4[2].x, a4[2].y, a4[2].z, a4[2].w, a4[3].x, a4[3].y, a4[3].z, a4[3].w};
     const uint32_t dd[4] = {d4.x, d4.y, d4.z, d4.w};
 #pragma unroll
     for (int k = 0; k < 16; ++k) {
@@ -679,7 +687,7 @@ __device__ int visit_label(const uint8_t* __restrict__ adm, K* key, uint16_t* ls
         const uint4 q = k4[k >> 2];
         sK[r0 + k] = (k & 3) == 0 ? q.x : ((k & 3) == 1 ? q.y : ((k & 3) == 2 ? q.z : q.w));
       }
-      if (WITH_SET) sA[r0 + k] = (uint16_t)((k & 1) ? (aa[k >> 1] >> 16) : (aa[k >> 1] & 0xffffu));
+      if (WITH_SET) sA[r0 + k] = aa[k];
       sD[r0 + k] = (uint8_t)((dd[k >> 2] >> (8 * (k & 3))) & 0xffu);
     }
 #pragma unroll
@@ -692,7 +700,7 @@ for (int i = tid; i < kH * kH * kH; i += kThreads) {
       if (nh > 1) continue;
       const long long p = flat_or_invalid(g, t.z0 + hz - 1, t.y0 + hy - 1, t.x0 + hx - 1);
       K k = KeyT<K>::inf;
-      uint16_t s = kSetEmpty;
+      uint32_t s = kSetEmpty;
       uint8_t d = 0;
       if (p >= 0) {
         k = __ldcg(&key[p]);
@@ -711,17 +719,17 @@ for (int i = tid; i < kH * kH * kH; i += kThreads) {
   auto line = [&](int base, int s, int len, uint32_t from_lo, uint32_t from_hi, bool& ch, bool& first, bool& last) {
     {
       K kp = sK[base - s];
-      uint16_t ap = WITH_SET ? sA[base - s] : kSetEmpty;
+      uint32_t ap = WITH_SET ? sA[base - s] : kSetEmpty;
       for (int j = 0; j < len; ++j) {
         const int idx = base + j * s;
         K k = sK[idx];
-        uint16_t av = WITH_SET ? sA[idx] : kSetEmpty;
+        uint32_t av = WITH_SET ? sA[idx] : kSetEmpty;
         if ((sD[idx] & from_lo) && kp != KeyT<K>::inf) {
           bool c = false;
           const K cand = kp + KeyT<K>::hop;
           if (cand < k) { k = cand; sK[idx] = k; c = true; }
           if (WITH_SET && ap != kSetEmpty) {
-            const uint16_t j1 = set_join(av, ap);
+            const uint32_t j1 = set_join(av, ap);
             if (j1 != av) { av = j1; sA[idx] = av; c = true; }
           }
           if (c) { ch = true; first |= j == 0; last |= j == len - 1; }
@@ -731,17 +739,17 @@ for (int i = tid; i < kH * kH * kH; i += kThreads) {
     }
     {
       K kp = sK[base + len * s];
-      uint16_t ap = WITH_SET ? sA[base + len * s] : kSetEmpty;
+      uint32_t ap = WITH_SET ? sA[base + len * s] : kSetEmpty;
       for (int j = len - 1; j >= 0; --j) {
         const int idx = base + j * s;
         K k = sK[idx];
-        uint16_t av = WITH_SET ? sA[idx] : kSetEmpty;
+        uint32_t av = WITH_SET ? sA[idx] : kSetEmpty;
         if ((sD[idx] & from_hi) && kp != KeyT<K>::inf) {
           bool c = false;
           const K cand = kp + KeyT<K>::hop;
           if (cand < k) { k = cand; sK[idx] = k; c = true; }
           if (WITH_SET && ap != kSetEmpty) {
-            const uint16_t j1 = set_join(av, ap);
+            const uint32_t j1 = set_join(av, ap);
             if (j1 != av) { av = j1; sA[idx] = av; c = true; }
           }
           if (c) { ch = true; first |= j == 0; last |= j == len - 1; }
@@ -815,12 +823,8 @@ for (int i = tid; i < kH * kH * kH; i += kThreads) {
     }
     if (WITH_SET) {
 #pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        uint32_t v[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) v[q] = (uint32_t)sA[c0 + 8 * k + 2 * q] | ((uint32_t)sA[c0 + 8 * k + 2 * q + 1] << 16);
-        __stcg((uint4*)(lset + p0) + k, make_uint4(v[0], v[1], v[2], v[3]));
-      }
+      for (int k = 0; k < 4; ++k)
+        __stcg((uint4*)(lset + p0) + k, make_uint4(sA[c0 + 4 * k], sA[c0 + 4 * k + 1], sA[c0 + 4 * k + 2], sA[c0 + 4 * k + 3]));
     }
   } else if (a < t.vy && b + 1 >= t.uz0 && b + 1 < t.uz1) {
     const long long p0 = ((long long)(t.z0 + b) * g.ny + (t.y0 + a)) * g.nx + t.x0;
@@ -841,21 +845,29 @@ for (int i = tid; i < kH * kH * kH; i += kThreads) {
 // L.cnt[5] rounds.
 template <int PHASE, int MODE, bool WITH_SET, typename K>
 __global__ void __launch_bounds__(kThreads, (PHASE == 1 || !WITH_SET || sizeof(K) == 4) ? 3 : 2)
-    k_wsf_persistent(const uint16_t* __restrict__ img, uint32_t* cost, K* key, uint16_t* lset,
+    k_wsf_persistent(const uint16_t* __restrict__ img, uint32_t* cost, K* key, uint32_t* lset,
                      const uint8_t* __restrict__ adm, FGrid g, Lists L, int max_rounds) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ unsigned long long s_raw[];
   __shared__ int s_faces;
-  // phase 1: cost u32 + intensity u16; phase 2: key (u64 or u32) + set u16 + admissibility u8
+  // phase 1: cost u32 + intensity u16; phase 2: key (u64 or u32) + set u32 + admissibility u8
   uint32_t* sC = (uint32_t*)s_raw;
   uint16_t* sI = (uint16_t*)(sC + kCells);
   K* sK = (K*)s_raw;
-  uint16_t* sA = (uint16_t*)(sK + kCells);
+  uint32_t* sA = (uint32_t*)(sK + kCells);
   uint8_t* sD = WITH_SET ? (uint8_t*)(sA + kCells) : (uint8_t*)(sK + kCells);
   const int tid = threadIdx.x;
   int r = 0;
   for (;; ++r) {
     const int cur = r % 3, nxt = (r + 1) % 3, old = (r + 2) % 3;
+    // 32-bit keys: a hop count that reached kKeyFull32 in the last round ends the phase at this
+    // barrier (the host re-runs it on 64-bit keys; relaxing on would wrap keys modulo 2^32). The
+    // flag of round r lives in cnt[8 + (r & 1)]: written during round r only, read by every block
+    // between the barriers of rounds r and r + 1, so all blocks take the same decision.
+    if (sizeof(K) == 4 && r > 0 && __ldcg(&L.cnt[8 + ((r - 1) & 1)]) != 0) {
+      if (blockIdx.x == 0 && tid == 0) { L.cnt[4] = 2; atomicAdd(&g_stats[7], 1); }
+      break;
+    }
     const int n = __ldcg(&L.cnt[cur]);
     if (n == 0) break;
     if (r >= max_rounds) { if (blockIdx.x == 0 && tid == 0) L.cnt[4] = 1; break; }
@@ -868,11 +880,11 @@ __global__ void __launch_bounds__(kThreads, (PHASE == 1 || !WITH_SET || sizeof(K
       if (t.uz0 >= t.uz1) continue;
       int res;
       if (PHASE == 1) res = visit_cost<MODE>(img, cost, g, t, sC, sI, &s_faces);
-      else res = visit_label<K, WITH_SET>(adm, key, lset, g, t, sK, sA, sD, &s_faces, &L.cnt[4]);
+      else res = visit_label<K, WITH_SET>(adm, key, lset, g, t, sK, sA, sD, &s_faces, &L.cnt[8 + (r & 1)]);
       if (res) {
         __threadfence();
         post_neighbours(g, L, nxt, t, s_faces);
-        if (res == 2 && tid == 32) post_tile(L, g.ntiles, nxt, tile);
+        if (res == 2 && tid == 32) { post_tile(L, g.ntiles, nxt, tile); atomicAdd(&g_stats[3], 1); }
       }
       __syncthreads();   // the shared tile is reused by the next visit
     }
@@ -882,7 +894,7 @@ __global__ void __launch_bounds__(kThreads, (PHASE == 1 || !WITH_SET || sizeof(K
 }
 
 __global__ void __launch_bounds__(256) k_wsf_labels(const unsigned long long* __restrict__ key,
-                                                    const uint16_t* __restrict__ lset, long long n,
+                                                    const uint32_t* __restrict__ lset, long long n,
                                                     int16_t* __restrict__ labels, uint8_t* __restrict__ ambiguous) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -896,7 +908,7 @@ __global__ void __launch_bounds__(256) k_wsf_labels(const unsigned long long* __
 // what = 0: cost (uint32 per voxel); what = 1: key (uint64) followed by the label sets (uint16)
 __global__ void __launch_bounds__(256) k_wsf_plane_get(const uint32_t* __restrict__ cost,
                                                        const unsigned long long* __restrict__ key,
-                                                       const uint16_t* __restrict__ lset, FGrid g, int z, int what,
+                                                       const uint32_t* __restrict__ lset, FGrid g, int z, int what,
                                                        void* out) {
   const int pn = g.ny * g.nx;
   const long long base = (long long)z * pn;
@@ -904,12 +916,12 @@ __global__ void __launch_bounds__(256) k_wsf_plane_get(const uint32_t* __restric
     if (what == 0) ((uint32_t*)out)[i] = cost[base + i];
     else {
       ((unsigned long long*)out)[i] = key[base + i];
-      ((uint16_t*)((unsigned long long*)out + pn))[i] = lset[base + i];
+      ((uint32_t*)((unsigned long long*)out + pn))[i] = lset[base + i];
     }
   }
 }
 
-__global__ void __launch_bounds__(256) k_wsf_plane_merge(uint32_t* cost, unsigned long long* key, uint16_t* lset,
+__global__ void __launch_bounds__(256) k_wsf_plane_merge(uint32_t* cost, unsigned long long* key, uint32_t* lset,
                                                          FGrid g, int z, int what, const void* in, Lists L) {
   const int pn = g.ny * g.nx;
   const long long base = (long long)z * pn;
@@ -920,10 +932,10 @@ __global__ void __launch_bounds__(256) k_wsf_plane_merge(uint32_t* cost, unsigne
       if (v < cost[base + i]) { cost[base + i] = v; ch = true; }
     } else {
       const unsigned long long k = ((const unsigned long long*)in)[i];
-      const uint16_t s = ((const uint16_t*)((const unsigned long long*)in + pn))[i];
+      const uint32_t s = ((const uint32_t*)((const unsigned long long*)in + pn))[i];
       if (k < key[base + i]) { key[base + i] = k; ch = true; }
       if (s != kSetEmpty) {
-        const uint16_t j = set_join(lset[base + i], s);
+        const uint32_t j = set_join(lset[base + i], s);
         if (j != lset[base + i]) { lset[base + i] = j; ch = true; }
       }
     }
@@ -950,7 +962,7 @@ int launch_persistent(K kern, size_t smem, const uint16_t* img, FastWs& w, FGrid
   if (grid > g.ntiles) grid = g.ntiles;
   uint32_t* cost = w.cost;
   void* key = keyptr ? keyptr : (void*)w.key;
-  uint16_t* lset = w.lset;
+  uint32_t* lset = w.lset;
   const uint8_t* adm = w.adm;
   Lists L = w.L;
   int max_rounds = 1 << 20;
@@ -1029,7 +1041,7 @@ int b2v_wsf_run(int stages, const uint16_t* img, const int16_t* markers, int64_t
   if ((stages & 8) && use32) {
     k_wsf_key32_init<<<b2v_grid(g.n, 256 * 4, 16), 256, 0, s>>>(w.key, g.n, w.present, w.prefix, w.key32);
     if ((rc = b2v_check_launch("k_wsf_key32_init"))) return rc;
-    const size_t smem = (size_t)kCells * (with_set ? 7 : 5) + 16;
+    const size_t smem = (size_t)kCells * (with_set ? 9 : 5) + 16;
     rc = with_set ? launch_persistent(k_wsf_persistent<2, 0, true, uint32_t>, smem, img, w, g, s, w.key32)
                   : launch_persistent(k_wsf_persistent<2, 0, false, uint32_t>, smem, img, w, g, s, w.key32);
     if (rc) return rc;
@@ -1043,7 +1055,7 @@ int b2v_wsf_run(int stages, const uint16_t* img, const int16_t* markers, int64_t
     }
   }
   if ((stages & 8) && !use32) {
-    const size_t smem = (size_t)kCells * (with_set ? 11 : 9) + 16;
+    const size_t smem = (size_t)kCells * (with_set ? 13 : 9) + 16;
     rc = with_set ? launch_persistent(k_wsf_persistent<2, 0, true, unsigned long long>, smem, img, w, g, s)
                   : launch_persistent(k_wsf_persistent<2, 0, false, unsigned long long>, smem, img, w, g, s);
     if (rc) return rc;
@@ -1075,7 +1087,7 @@ extern "C" int b2v_ws_stats(int* out8, int reset) {
 }
 
 extern "C" int64_t b2v_ws_plane_bytes(int64_t ny, int64_t nx, int what) {
-  return what == 0 ? ny * nx * 4 : ny * nx * 10;
+  return what == 0 ? ny * nx * 4 : ny * nx * 12;
 }
 
 extern "C" int b2v_ws_plane(int merge, int what, int64_t nz, int64_t ny, int64_t nx, int mode, int frozen_lo,

@@ -333,3 +333,161 @@ int orc_ift_scipy(const uint16_t* image, const int16_t* markers, int64_t nz, int
   free(nxt); free(prv); free(cost); free(done); free(queued); free(first); free(last);
   return 0;
 }
+
+/* ------------------------------------------------------------------------------------------
+ * orc_ws_labels — the device engines' complete labelling rule (b2v_ws_flood, DESIGN.md §6) in
+ * O(N), so that every voxel of large volumes can be checked, ambiguous ones included (TEST
+ * INFRASTRUCTURE). Same cost model and admissibility as orc_ws_model / tests/ws_model.py:
+ *   1. C = exact minimax cost, by a bucket-queue Dijkstra (Dial: costs are uint16 values and a
+ *      path's cost never decreases along it, so buckets are popped in increasing order);
+ *   2. v -> p admissible: p is no marker, C(p) and C(v) finite and
+ *        mode 0: max(C(v), |I(v) - I(p)|) == C(p);   mode 1: C(v) == min over p's neighbours of C;
+ *   3. key (hops, code), code = label + 32768: breadth-first over admissible edges from the
+ *      markers (hops 0, own code), in hop order; a voxel first seen at hop h + 1 takes the smallest
+ *      code among its admissible predecessors at hop h (the minimum of hops << 32 | code);
+ *   4. ambiguous: two different labels reach p along admissible edges (least fixed point of the
+ *      label-set join, by a worklist: a set changes at most twice, empty -> one label -> several).
+ * labels_out int16 (0 where no marker reaches); amb_out uint8; hops_out uint32 (optional, may be
+ * NULL; 0xffffffff where unreached). Returns 0, or -1 if memory runs out.
+ * ------------------------------------------------------------------------------------------ */
+int orc_ws_labels(const uint16_t* image, const int16_t* markers, int64_t nz, int64_t ny, int64_t nx,
+                  const uint8_t* strct, int64_t sz, int64_t sy, int64_t sx, int mode, int16_t* labels_out,
+                  uint8_t* amb_out, uint32_t* hops_out) {
+  const int64_t n = nz * ny * nx;
+  const uint32_t INF = 0xffffffffu;
+  int64_t noff = 0, off[27][3];
+  for (int64_t k = 0; k < sz; ++k)
+    for (int64_t j = 0; j < sy; ++j)
+      for (int64_t i = 0; i < sx; ++i)
+        if (strct[(k * sy + j) * sx + i]) {
+          int64_t dz = k - sz / 2, dy = j - sy / 2, dx = i - sx / 2;
+          if (dz == 0 && dy == 0 && dx == 0) continue;
+          off[noff][0] = dz; off[noff][1] = dy; off[noff][2] = dx;
+          ++noff;
+        }
+#define WL_NB(p, o, sign, q)                                                                          \
+  do {                                                                                                \
+    if (mode == 0) {                                                                                  \
+      int64_t qq = (p) + (sign) * ((off[o][0] * ny + off[o][1]) * nx + off[o][2]);                    \
+      (q) = (qq >= 0 && qq < n) ? qq : -1;                                                            \
+    } else {                                                                                          \
+      int64_t z_ = (p) / (ny * nx), r_ = (p) % (ny * nx), y_ = r_ / nx, x_ = r_ % nx;                 \
+      int64_t zz = z_ + (sign)*off[o][0], yy = y_ + (sign)*off[o][1], xx = x_ + (sign)*off[o][2];     \
+      (q) = (zz >= 0 && zz < nz && yy >= 0 && yy < ny && xx >= 0 && xx < nx) ? (zz * ny + yy) * nx + xx : -1; \
+    }                                                                                                 \
+  } while (0)
+  uint32_t* cost = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)n);
+  int64_t* nxt = (int64_t*)malloc(sizeof(int64_t) * (size_t)n);
+  int64_t* prv = (int64_t*)malloc(sizeof(int64_t) * (size_t)n);
+  int64_t* head = (int64_t*)malloc(sizeof(int64_t) * 65536);
+  if (!cost || !nxt || !prv || !head) { free(cost); free(nxt); free(prv); free(head); return -1; }
+  /* ---- 1. costs: one doubly linked list per cost value; a voxel is in at most one list */
+  for (int b = 0; b < 65536; ++b) head[b] = -1;
+#define WL_PUSH(p, b) do { prv[p] = -1; nxt[p] = head[b]; if (head[b] >= 0) prv[head[b]] = (p); head[b] = (p); } while (0)
+#define WL_UNLINK(p, b) do { if (prv[p] >= 0) nxt[prv[p]] = nxt[p]; else head[b] = nxt[p]; if (nxt[p] >= 0) prv[nxt[p]] = prv[p]; } while (0)
+  for (int64_t p = 0; p < n; ++p) {
+    if (markers[p]) {
+      cost[p] = mode == 0 ? 0u : (uint32_t)image[p];
+      WL_PUSH(p, cost[p]);
+    } else cost[p] = INF;
+  }
+  for (int64_t b = 0; b < 65536; ++b)
+    while (head[b] >= 0) {
+      const int64_t v = head[b];
+      head[b] = nxt[v];
+      if (head[b] >= 0) prv[head[b]] = -1;
+      for (int64_t o = 0; o < noff; ++o) {
+        int64_t p;
+        WL_NB(v, o, 1, p);
+        if (p < 0 || markers[p]) continue;
+        const uint32_t w = mode == 0 ? (uint32_t)abs((int)image[v] - (int)image[p]) : (uint32_t)image[p];
+        const uint32_t cand = (uint32_t)b > w ? (uint32_t)b : w;
+        if (cand < cost[p]) {      /* cand >= b: p is in a bucket not yet popped, or in none */
+          if (cost[p] != INF) WL_UNLINK(p, cost[p]);
+          cost[p] = cand;
+          WL_PUSH(p, cand);
+        }
+      }
+    }
+#undef WL_PUSH
+#undef WL_UNLINK
+  free(nxt); free(prv); free(head);
+  /* the cost an admissible predecessor offers: mode 0 C(p) itself, mode 1 the smallest C among p's
+   * neighbours (the voxels u with p = u + offset) */
+  uint32_t* want = cost;
+  if (mode == 1) {
+    want = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)n);
+    if (!want) { free(cost); return -1; }
+    for (int64_t p = 0; p < n; ++p) {
+      uint32_t cmin = INF;
+      for (int64_t o = 0; o < noff; ++o) {
+        int64_t u;
+        WL_NB(p, o, -1, u);
+        if (u >= 0 && cost[u] < cmin) cmin = cost[u];
+      }
+      want[p] = cmin;
+    }
+  }
+#define WL_ADM(v, p)                                                                                  \
+  (!markers[p] && cost[p] != INF && cost[v] != INF &&                                                 \
+   (mode == 0 ? ((cost[v] > (uint32_t)abs((int)image[v] - (int)image[p]) ? cost[v]                    \
+                                                                          : (uint32_t)abs((int)image[v] - (int)image[p])) == cost[p]) \
+              : cost[v] == want[p]))
+  /* ---- 3. keys: breadth-first in hop order */
+  uint32_t* hops = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)n);
+  uint16_t* code = (uint16_t*)malloc(sizeof(uint16_t) * (size_t)n);
+  int64_t* queue = (int64_t*)malloc(sizeof(int64_t) * (size_t)n);
+  if (!hops || !code || !queue) {
+    free(hops); free(code); free(queue); if (want != cost) free(want); free(cost);
+    return -1;
+  }
+  int64_t qh = 0, qt = 0;
+  for (int64_t p = 0; p < n; ++p) {
+    if (markers[p]) { hops[p] = 0; code[p] = (uint16_t)(markers[p] + 32768); queue[qt++] = p; }
+    else { hops[p] = INF; code[p] = 0; }
+  }
+  while (qh < qt) {
+    const int64_t v = queue[qh++];
+    for (int64_t o = 0; o < noff; ++o) {
+      int64_t p;
+      WL_NB(v, o, 1, p);
+      if (p < 0 || !WL_ADM(v, p)) continue;
+      if (hops[p] == INF) { hops[p] = hops[v] + 1; code[p] = code[v]; queue[qt++] = p; }
+      else if (hops[p] == hops[v] + 1 && code[v] < code[p]) code[p] = code[v];
+    }
+  }
+  for (int64_t p = 0; p < n; ++p) labels_out[p] = hops[p] == INF ? 0 : (int16_t)((int)code[p] - 32768);
+  if (hops_out) memcpy(hops_out, hops, sizeof(uint32_t) * (size_t)n);
+  free(hops); free(code);
+  /* ---- 4. label sets: -1 empty, -2 two different labels, else the one label's code */
+  int32_t* set = (int32_t*)malloc(sizeof(int32_t) * (size_t)n);
+  uint8_t* inq = (uint8_t*)calloc((size_t)n, 1);
+  if (!set || !inq) { free(set); free(inq); free(queue); if (want != cost) free(want); free(cost); return -1; }
+  int64_t qn = 0;
+  qh = qt = 0;
+  for (int64_t p = 0; p < n; ++p) {
+    set[p] = markers[p] ? (int32_t)markers[p] + 32768 : -1;
+    if (markers[p]) { queue[qt] = p; qt = (qt + 1) % n; ++qn; inq[p] = 1; }
+  }
+  while (qn) {
+    const int64_t v = queue[qh]; qh = (qh + 1) % n; --qn; inq[v] = 0;
+    const int32_t sv = set[v];
+    for (int64_t o = 0; o < noff; ++o) {
+      int64_t p;
+      WL_NB(v, o, 1, p);
+      if (p < 0 || !WL_ADM(v, p)) continue;
+      const int32_t sp = set[p], ns = sp == -1 ? sv : (sp == sv ? sp : -2);
+      if (ns != sp) {
+        set[p] = ns;
+        if (!inq[p]) { queue[qt] = p; qt = (qt + 1) % n; ++qn; inq[p] = 1; }
+      }
+    }
+  }
+  for (int64_t p = 0; p < n; ++p) amb_out[p] = set[p] == -2;
+#undef WL_ADM
+#undef WL_NB
+  free(set); free(inq); free(queue);
+  if (want != cost) free(want);
+  free(cost);
+  return 0;
+}

@@ -90,3 +90,29 @@ def ift_scipy_restated(image_u16, markers_i16, bstruct, quirk=True):
     lib().orc_ift_scipy(_ptr(img), _ptr(mk), *map(C.c_int64, img.shape), _ptr(st), *map(C.c_int64, st.shape),
                         C.c_int(1 if quirk else 0), _ptr(out), C.byref(sole))
     return out.reshape(np.shape(image_u16)), sole.value
+
+
+def ws_labels(image_u16, markers_i16, bstruct, mode, return_hops=False):
+    """oracle/watershed.c::orc_ws_labels — the device flood's complete labelling rule (b2v_ws_flood,
+    DESIGN.md section 6) in O(N): labels (int16: fewest hops along cost-optimal edges, then the
+    smaller label; 0 unreached) and the ambiguous mask (uint8: two different labels reach the voxel
+    along cost-optimal edges); with return_hops also the hop counts (uint32, 0xffffffff unreached).
+    Any structuring element; mode 0 = watershed_ift's cost and flat-array neighbourhood, mode 1 =
+    skimage's cost, proper bounds."""
+    img = np.ascontiguousarray(image_u16, dtype=np.uint16)
+    mk = np.ascontiguousarray(markers_i16, dtype=np.int16)
+    st = np.ascontiguousarray(bstruct, dtype=np.uint8)
+    if img.ndim == 2:
+        img, mk, st = img[None], mk[None], st[None]
+    if img.shape != mk.shape or st.ndim != 3:
+        raise ValueError("ws_labels: image and markers must share a 3-D shape, with a 3-D structure")
+    labels = np.empty(img.shape, np.int16)
+    amb = np.empty(img.shape, np.uint8)
+    hops = np.empty(img.shape, np.uint32) if return_hops else None
+    rc = lib().orc_ws_labels(_ptr(img), _ptr(mk), *map(C.c_int64, img.shape), _ptr(st), *map(C.c_int64, st.shape),
+                             C.c_int(mode), _ptr(labels), _ptr(amb), _ptr(hops) if return_hops else None)
+    if rc != 0:
+        raise MemoryError("ws_labels: out of memory")
+    shape = np.shape(image_u16)
+    out = (labels.reshape(shape), amb.reshape(shape))
+    return out + (hops.reshape(shape),) if return_hops else out

@@ -13,7 +13,7 @@ import numpy as np
 INF_C = np.uint32(0xFFFFFFFF)
 INF_K = np.uint64(0xFFFFFFFFFFFFFFFF)
 HOP = np.uint64(1 << 32)
-EMPTY, MULTI = 32768, 0
+EMPTY, MULTI = 32768, 0x10000      # label sets as the engines store them (uint32): label + 32768, or these
 
 
 def _shifted(a, off, fill, mode, shape):
