@@ -115,9 +115,32 @@ static inline int64_t align256(int64_t bytes) { return (bytes + 255) & ~(int64_t
 __device__ __forceinline__ int64_t gtid() { return (int64_t)blockIdx.x * blockDim.x + threadIdx.x; }
 __device__ __forceinline__ int64_t gstride() { return (int64_t)gridDim.x * blockDim.x; }
 
-// Block-wide exclusive scan: returns x's prefix and stores the block total. Every thread of the block calls
-// it; blockDim.x is a multiple of 32, and s_w holds blockDim.x / 32 words.
+namespace {
+// a[0, n) = v, grid-stride (each translation unit has its own instantiations)
 template <typename T>
+__global__ void __launch_bounds__(256) k_fill(T* a, int64_t n, T v) {
+  for (int64_t i = gtid(); i < n; i += gstride()) a[i] = v;
+}
+}  // namespace
+
+// Block-wide sum of a block of 256 threads, returned to thread 0 (the other threads get 0). Every thread of
+// the block calls it; s_w holds 8 words.
+template <typename T>
+__device__ __forceinline__ T block_sum(T x, T* s_w) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = x;
+  __syncthreads();
+  T t = 0;
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 8; ++k) t += s_w[k];
+  return t;
+}
+
+// Block-wide exclusive scan: returns x's prefix and stores the block total. Every thread of the block calls
+// it; blockDim.x is a multiple of 32, and s_w holds blockDim.x / 32 words. A kernel whose blocks have fewer
+// than 32 warps may say so in MaxWarps (a power of two), which shortens the scan of the warp sums.
+template <typename T, int MaxWarps = 32>
 __device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   T inc = x;
@@ -130,7 +153,7 @@ __device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
   if (wid == 0) {
     const int nw = blockDim.x >> 5;
     T v = lane < nw ? s_w[lane] : 0;
-    for (int o = 1; o < 32; o <<= 1) {
+    for (int o = 1; o < MaxWarps; o <<= 1) {
       const T y = __shfl_up_sync(0xffffffffu, v, o);
       if (lane >= o) v += y;
     }
@@ -142,6 +165,24 @@ __device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
   __syncthreads();
   return base + inc - x;
 }
+
+// ---- 3x3x3 structuring elements ---------------------------------------------------------
+// A uint8 element [odz][ody][odx] of at most 3 voxels on each axis, centred at (odz / 2, ody / 2, odx / 2), as
+// a 27-bit mask: bit (oz+1)*9 + (oy+1)*3 + (ox+1) stands for the offset (oz, oy, ox); bit 13 is the centre.
+static inline uint32_t strct_mask(const uint8_t* st, int64_t odz, int64_t ody, int64_t odx) {
+  uint32_t sb = 0;
+  for (int64_t kk = 0; kk < odz; ++kk)
+    for (int64_t jj = 0; jj < ody; ++jj)
+      for (int64_t ii = 0; ii < odx; ++ii)
+        if (st[(kk * ody + jj) * odx + ii]) {
+          const int oz = (int)(kk - odz / 2), oy = (int)(jj - ody / 2), ox = (int)(ii - odx / 2);
+          sb |= 1u << ((oz + 1) * 9 + (oy + 1) * 3 + (ox + 1));
+        }
+  return sb;
+}
+
+// the six face neighbours (0,0,+-1), (0,+-1,0), (+-1,0,0): generate_binary_structure(3, 1) without its centre
+constexpr uint32_t kSB6 = (1u << 12) | (1u << 14) | (1u << 10) | (1u << 16) | (1u << 4) | (1u << 22);
 
 // ---- triangle faces ---------------------------------------------------------------
 // int32 or int64 ids, [T,3] or [T,4] with a leading 3 (the Mesh form), every id in [0, nv)

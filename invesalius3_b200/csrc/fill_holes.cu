@@ -46,7 +46,6 @@ namespace cg = cooperative_groups;
 
 namespace {
 
-constexpr int kMaxBlocksPerSm = 2;
 enum : int8_t { FILLED = 0, FAILED = 1, TOO_LARGE = 2 };
 
 struct FhWs {
@@ -546,15 +545,6 @@ __global__ void __launch_bounds__(kBlock) k_fh_out(const int32_t* __restrict__ f
   }
 }
 
-int launch_coop(const void* fn, void** args, cudaStream_t s, const char* what) {
-  int per_sm = 0;
-  B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlock, 0));
-  B2V_REQUIRE(per_sm >= 1, B2V_ERR_CUDA, "fill_holes: %s does not fit on an SM", what);
-  if (per_sm > kMaxBlocksPerSm) per_sm = kMaxBlocksPerSm;
-  B2V_CUDA(cudaLaunchCooperativeKernel(fn, dim3(per_sm * b2v_sm_count()), dim3(kBlock), args, 0, s));
-  return b2v_check_launch(what);
-}
-
 int check_sizes(int64_t nv, int64_t nt, const char* what) {
   B2V_REQUIRE(nv >= 0 && nv <= 0x7fffffffLL && nt >= 0 && nt <= 0x7fffffffLL / 6, B2V_ERR_ARG,
               "%s: need V < 2^31 and 6T < 2^31", what);
@@ -614,7 +604,7 @@ extern "C" int b2v_holes_count(const float* verts, int64_t nv, const void* faces
   if (int rc = b2v_check_launch("k_fh_darts")) return rc;
   Pj J{{w.nx[0], w.nx[1]}, {w.dd[0], w.dd[1]}, {w.mn[0], w.mn[1]}, {w.last[0], w.last[1]}, w.ctl};
   void* args[] = {&J};
-  if (int rc = launch_coop((const void*)k_fh_jump, args, s, "k_fh_jump")) return rc;
+  if (int rc = launch_coop((const void*)k_fh_jump, args, s, "fill_holes", "k_fh_jump")) return rc;
   B2V_CUDA(cudaMemsetAsync(w.lkey, 0, (size_t)(L + 1) * 8, s));
   k_fh_loops<<<gd, kBlock, 0, s>>>(w.lines, w.deg, w.succ, J, w.lkey, w.lsd, w.lterm);
   if (int rc = b2v_check_launch("k_fh_loops")) return rc;

@@ -337,7 +337,6 @@ __device__ __forceinline__ int sweep_column(uint32_t* sR, const uint32_t* sF, in
 // SBC != 0 fixes the structuring element at compile time (6-, 18-, 26-connectivity): the
 // stencil loops lose their dead rows and, for axis-only elements, the generic hop vanishes
 // (the three sweeps already cover every offset).
-constexpr uint32_t kSB6 = (1u << 12) | (1u << 14) | (1u << 10) | (1u << 16) | (1u << 4) | (1u << 22);
 constexpr uint32_t kSB26 = 0x7ffffffu & ~(1u << 13);
 constexpr uint32_t kSB18 = kSB26 & ~((1u << 0) | (1u << 2) | (1u << 6) | (1u << 8) | (1u << 18) | (1u << 20) |
                                      (1u << 24) | (1u << 26));
@@ -1073,16 +1072,9 @@ int strct_bits(const uint8_t* strct_host, int64_t odz, int64_t ody, int64_t odx,
   B2V_REQUIRE(odz <= 3 && ody <= 3 && odx <= 3, B2V_ERR_ARG,
               "floodfill: structuring elements larger than 3x3x3 are not supported (got %lldx%lldx%lld)",
               (long long)odz, (long long)ody, (long long)odx);
-  uint32_t bits = 0;
-  for (int64_t kk = 0; kk < odz; ++kk)
-    for (int64_t jj = 0; jj < ody; ++jj)
-      for (int64_t ii = 0; ii < odx; ++ii)
-        if (strct_host[(kk * ody + jj) * odx + ii]) {
-          int oz = (int)(kk - odz / 2), oy = (int)(jj - ody / 2), ox = (int)(ii - odx / 2);
-          bits |= 1u << ((oz + 1) * 9 + (oy + 1) * 3 + (ox + 1));
-        }
-  *sb = bits & ~(1u << 13);   // the centre offset moves nothing: drop it so that the standard elements
-                              // match the compile-time specialisations
+  // the centre offset moves nothing: drop it so that the standard elements match the compile-time
+  // specialisations
+  *sb = strct_mask(strct_host, odz, ody, odx) & ~(1u << 13);
   return B2V_OK;
 }
 
@@ -1371,8 +1363,7 @@ extern "C" int b2v_floodfill_threshold_inplace(void* data, int dtype, int64_t dz
 extern "C" int b2v_floodfill_equal(const void* data, int dtype, int64_t dz, int64_t dy, int64_t dx, int64_t i,
                                    int64_t j, int64_t k, double v, uint8_t fill, uint8_t* out, void* workspace,
                                    void* stream, int* rounds_out) {
-  // 6-connected: (0,0,+-1), (0,+-1,0), (+-1,0,0)
-  const uint32_t sb = (1u << 12) | (1u << 14) | (1u << 10) | (1u << 16) | (1u << 4) | (1u << 22);
+  const uint32_t sb = kSB6;
   int64_t seed[3] = {i, j, k};
   if (rounds_out) *rounds_out = 0;
   return flood_dispatch<MODE_EQUAL>(const_cast<void*>(data), dtype, out, dz, dy, dx, seed, 1, v, v, 0.0, fill, sb,

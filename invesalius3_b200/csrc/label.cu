@@ -10,6 +10,7 @@
 // Labels are then numbered in the order of the components' first voxel in raster order, which is
 // SciPy's numbering: roots are flagged, an exclusive scan over the flags ranks them.
 #include "b2v_common.cuh"
+#include "scan.cuh"
 
 namespace {
 
@@ -100,58 +101,15 @@ __global__ void __launch_bounds__(256) k_label_flatten_count(const int* __restri
       labels[i] = r;
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int k = 0; k < 8; ++k) t += s[k];
-    bsum[blockIdx.x] = t;
-  }
-}
-
-// exclusive scan of the block sums by one block; total -> bsum[nb]
-__global__ void __launch_bounds__(1024) k_label_scan_bsums(uint32_t* bsum, long long nb) {
-  __shared__ uint32_t s_w[32];
-  __shared__ uint32_t s_carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (long long b0 = 0; b0 < nb; b0 += 1024) {
-    const long long i = b0 + tid;
-    const uint32_t v = i < nb ? bsum[i] : 0u;
-    uint32_t incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += u;
-    }
-    if (lane == 31) s_w[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = s_w[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, w, o);
-        if (lane >= o) w += u;
-      }
-      s_w[lane] = w;
-    }
-    __syncthreads();
-    const uint32_t before = s_carry + (warp ? s_w[warp - 1] : 0u) + incl - v;
-    if (i < nb) bsum[i] = before;
-    __syncthreads();
-    if (tid == 1023) s_carry = before + v;
-    __syncthreads();
-  }
-  if (tid == 0) bsum[nb] = s_carry;
+  const uint32_t t = block_sum(c, s);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = t;
 }
 
 // roots get their number (rank in raster order + 1), stored in parent[] (no longer needed as a forest)
 __global__ void __launch_bounds__(256) k_label_number_roots(int* parent, LDims d, const uint32_t* __restrict__ bsum,
                                                             const uint32_t* __restrict__ labels) {
-  __shared__ uint32_t s[8];
+  __shared__ uint32_t s_w[8];
+  __shared__ uint32_t s_tot;
   const long long base = (long long)blockIdx.x * kScanBlock;
   uint32_t flags = 0, c = 0;
 #pragma unroll
@@ -159,17 +117,7 @@ __global__ void __launch_bounds__(256) k_label_number_roots(int* parent, LDims d
     const long long i = base + threadIdx.x * 8 + k;
     if (i < d.n && labels[i] == (uint32_t)i) { flags |= 1u << k; ++c; }
   }
-  uint32_t incl = c;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += u;
-  }
-  if (lane == 31) s[warp] = incl;
-  __syncthreads();
-  uint32_t before = bsum[blockIdx.x] + incl - c;
-  for (int k = 0; k < warp; ++k) before += s[k];
+  uint32_t before = bsum[blockIdx.x] + block_exscan(c, s_w, &s_tot);
 #pragma unroll
   for (int k = 0; k < 8; ++k)
     if ((flags >> k) & 1u) parent[base + threadIdx.x * 8 + k] = (int)(++before);
@@ -276,15 +224,8 @@ __global__ void __launch_bounds__(256) k_lb_count(const uint32_t* __restrict__ l
   int a, r;
 #pragma unroll
   for (int k = 0; k < 8; ++k) c += lb_emits(lo, hi, d, parent, rep, base + threadIdx.x * 8 + k, &a, &r);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int k = 0; k < 8; ++k) t += s[k];
-    bsum[blockIdx.x] = t;
-  }
+  const uint32_t t = block_sum(c, s);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = t;
 }
 
 // pairs[k] = (P(node), P(root of node)) in the order of the representatives (bsum: scanned block counts)
@@ -350,15 +291,8 @@ __global__ void __launch_bounds__(256) k_lr_flatten_count(const int* parent, int
       c += (r != (int)i);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int k = 0; k < 8; ++k) t += s[k];
-    bsum[blockIdx.x] = t;
-  }
+  const uint32_t t = block_sum(c, s);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = t;
 }
 
 // before[i] = |{non-roots at positions < i}| (bsum: scanned block counts)
@@ -417,19 +351,12 @@ __global__ void __launch_bounds__(256) k_label_relabel(uint32_t* labels, int64_t
   for (int64_t i = nv * 4 + gtid(); i < n; i += gstride()) labels[i] = map(labels[i]);
 }
 
-// sb: bit (oz+1)*9 + (oy+1)*3 + (ox+1) of a 1- or 3-wide structuring element; B2V_ERR_ARG (with SciPy's message
+// sb: the strct_mask of a 1- or 3-wide structuring element; B2V_ERR_ARG (with SciPy's message
 // where it has one) for any other shape or an asymmetric element
 int structure_bits(const uint8_t* strct_host, int64_t odz, int64_t ody, int64_t odx, uint32_t* sb_out) {
   B2V_REQUIRE(odz >= 1 && ody >= 1 && odx >= 1 && odz <= 3 && ody <= 3 && odx <= 3 && (odz & 1) && (ody & 1) && (odx & 1),
               B2V_ERR_ARG, "label: the structuring element must be 1 or 3 wide on every axis");
-  uint32_t sb = 0;
-  for (int64_t kk = 0; kk < odz; ++kk)
-    for (int64_t jj = 0; jj < ody; ++jj)
-      for (int64_t ii = 0; ii < odx; ++ii)
-        if (strct_host[(kk * ody + jj) * odx + ii]) {
-          const int oz = (int)(kk - odz / 2), oy = (int)(jj - ody / 2), ox = (int)(ii - odx / 2);
-          sb |= 1u << ((oz + 1) * 9 + (oy + 1) * 3 + (ox + 1));
-        }
+  const uint32_t sb = strct_mask(strct_host, odz, ody, odx);
   for (int o = 0; o < 13; ++o)     // SciPy: "structuring element is not symmetric"
     B2V_REQUIRE(((sb >> o) & 1u) == ((sb >> (26 - o)) & 1u), B2V_ERR_ARG, "label: structuring element is not symmetric");
   *sb_out = sb;
@@ -474,8 +401,8 @@ extern "C" int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t n
   if ((rc = b2v_check_launch("k_label_merge"))) return rc;
   k_label_flatten_count<<<(unsigned)nb, 256, 0, s>>>(parent, d, labels, bsum);
   if ((rc = b2v_check_launch("k_label_flatten_count"))) return rc;
-  k_label_scan_bsums<<<1, 1024, 0, s>>>(bsum, nb);
-  if ((rc = b2v_check_launch("k_label_scan_bsums"))) return rc;
+  k_scan_sums<uint32_t><<<1, 1024, 0, s>>>(bsum, nb, bsum + nb);
+  if ((rc = b2v_check_launch("k_scan_sums"))) return rc;
   k_label_number_roots<<<(unsigned)nb, 256, 0, s>>>(parent, d, bsum, labels);
   if ((rc = b2v_check_launch("k_label_number_roots"))) return rc;
   k_label_assign<<<b2v_grid(d.n, 256 * 4, 16), 256, 0, s>>>(parent, d, labels);
@@ -523,8 +450,8 @@ extern "C" int b2v_label_boundary_count(const uint32_t* lo_plane, const uint32_t
   if ((rc = b2v_check_launch("k_lb_unite"))) return rc;
   k_lb_count<<<(unsigned)L.nb, 256, 0, s>>>(lo_plane, hi_plane, d, L.parent, L.rep, L.bsum);
   if ((rc = b2v_check_launch("k_lb_count"))) return rc;
-  k_label_scan_bsums<<<1, 1024, 0, s>>>(L.bsum, L.nb);
-  if ((rc = b2v_check_launch("k_label_scan_bsums"))) return rc;
+  k_scan_sums<uint32_t><<<1, 1024, 0, s>>>(L.bsum, L.nb, L.bsum + L.nb);
+  if ((rc = b2v_check_launch("k_scan_sums"))) return rc;
   uint32_t total = 0;
   B2V_CUDA(cudaMemcpyAsync(&total, L.bsum + L.nb, 4, cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));
@@ -577,8 +504,8 @@ extern "C" int b2v_label_resolve(const int64_t* pairs, int64_t npairs, const int
     }
     k_lr_flatten_count<<<(unsigned)nb, 256, 0, s>>>(parent, nends, root, bsum);
     if ((rc = b2v_check_launch("k_lr_flatten_count"))) return rc;
-    k_label_scan_bsums<<<1, 1024, 0, s>>>(bsum, nb);
-    if ((rc = b2v_check_launch("k_label_scan_bsums"))) return rc;
+    k_scan_sums<uint32_t><<<1, 1024, 0, s>>>(bsum, nb, bsum + nb);
+    if ((rc = b2v_check_launch("k_scan_sums"))) return rc;
     k_lr_rank<<<(unsigned)nb, 256, 0, s>>>(root, nends, bsum, before);
     if ((rc = b2v_check_launch("k_lr_rank"))) return rc;
   } else {

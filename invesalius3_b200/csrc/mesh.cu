@@ -24,6 +24,7 @@
 // Bit-exact against the sequential CPU checker whenever no vertex receives offers from two seeds, and against
 // the round-by-round schedule of the NumPy restatement in tests/ca_smoothing_model.py.
 #include "b2v_common.cuh"
+#include "scan.cuh"
 
 namespace {
 
@@ -32,7 +33,7 @@ struct MeshWs {
   long long* last;      // [V]
   uint32_t* deg;        // [V + 1] adjacency degrees, then exclusive offsets
   uint32_t* adj;        // [6 M] neighbour ids (a triangle contributes at most two per vertex)
-  uint32_t* bsum;       // scan scratch
+  uint32_t* bsum;       // [scan_blocks(V + 1) + 1] scan scratch
   unsigned long long* dist;   // [V] squared distance bits
   int* seed;            // [V]
   int* frontier[2];     // [adjacency size] each
@@ -51,7 +52,7 @@ MeshWs carve(void* base, long long nv, long long nf) {
   w.last = (long long*)(p + off); off += align256(nv * 8);
   w.deg = (uint32_t*)(p + off); off += align256((nv + 1) * 4);
   w.adj = (uint32_t*)(p + off); off += align256(6 * nf * 4 + 4);
-  w.bsum = (uint32_t*)(p + off); off += align256((ceil_div64(nv + 1, 2048) + 2) * 4);
+  w.bsum = (uint32_t*)(p + off); off += align256((scan_blocks(nv + 1) + 1) * 4);
   w.dist = (unsigned long long*)(p + off); off += align256(nv * 8);
   w.seed = (int*)(p + off); off += align256(nv * 4);
   w.frontier[0] = (int*)(p + off); off += align256(6 * nf * 4 + nv * 4 + 4);
@@ -151,37 +152,6 @@ __global__ void __launch_bounds__(128) k_mesh_adjacency(const long long* __restr
   if (v >= nv || first[v] < 0) return;
   uint32_t* out = adj + off[v];
   for_each_neighbour(faces, order, first[v], last[v], v, [&](long long vj, int k) { out[k] = (uint32_t)vj; });
-}
-
-// exclusive scan of uint32 (in place), 2048 elements per block
-__global__ void __launch_bounds__(256) k_scan_reduce(const uint32_t* __restrict__ a, long long n, uint32_t* __restrict__ bsum) {
-  __shared__ uint32_t s[8];
-  const long long base = (long long)blockIdx.x * 2048;
-  uint32_t c = 0;
-  for (int k = 0; k < 8; ++k) { const long long i = base + threadIdx.x * 8 + k; if (i < n) c += a[i]; }
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int k = 0; k < 8; ++k) t += s[k]; bsum[blockIdx.x] = t; }
-}
-__global__ void k_scan_bsums(uint32_t* bsum, long long nb) {      // one thread: nb is small (V / 2048)
-  uint32_t run = 0;
-  for (long long i = 0; i < nb; ++i) { const uint32_t v = bsum[i]; bsum[i] = run; run += v; }
-  bsum[nb] = run;
-}
-__global__ void __launch_bounds__(256) k_scan_apply(uint32_t* a, long long n, const uint32_t* __restrict__ bsum) {
-  __shared__ uint32_t s[8];
-  const long long base = (long long)blockIdx.x * 2048;
-  uint32_t v[8], c = 0;
-  for (int k = 0; k < 8; ++k) { const long long i = base + threadIdx.x * 8 + k; v[k] = i < n ? a[i] : 0u; c += v[k]; }
-  uint32_t incl = c;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-  if (lane == 31) s[warp] = incl;
-  __syncthreads();
-  uint32_t run = bsum[blockIdx.x] + incl - c;
-  for (int k = 0; k < warp; ++k) run += s[k];
-  for (int k = 0; k < 8; ++k) { const long long i = base + threadIdx.x * 8 + k; if (i < n) a[i] = run; run += v[k]; }
 }
 
 // find_staircase_artifacts + the initial state of propagate_weights
@@ -289,14 +259,6 @@ __global__ void __launch_bounds__(256) k_mesh_step(float* pos, const double* __r
   pos[3 * i + 2] += (float)(wf * d[3 * i + 2]);
 }
 
-__global__ void k_fill_int(int* a, long long n, int v) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) a[i] = v;
-}
-__global__ void k_fill_i64(long long* a, long long n, long long v) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) a[i] = v;
-}
 // after a round: vertices claimed this round take their new seed; the marker array is reset
 __global__ void k_mesh_commit(int* seed, int* seed_new, const int* __restrict__ next, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -326,8 +288,8 @@ extern "C" int b2v_ca_smoothing(float* vertices, int64_t nverts, const int64_t* 
   int rc;
   B2V_CUDA(cudaMemsetAsync(w.status, 0, 4, s));
   B2V_CUDA(cudaMemsetAsync(w.fcount, 0, 16, s));
-  k_fill_i64<<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(w.first, nv, -1);
-  k_fill_int<<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(seed_new, nv, 0x7fffffff);
+  k_fill<long long><<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(w.first, nv, -1);
+  k_fill<int><<<(unsigned)ceil_div64(nv, 256), 256, 0, s>>>(seed_new, nv, 0x7fffffff);
   k_mesh_segments<<<b2v_grid(ne, 256, 32), 256, 0, s>>>((const long long*)faces4, (const long long*)order, ne, nv,
                                                         w.first, w.last, w.status);
   if ((rc = b2v_check_launch("k_mesh_segments"))) return rc;
@@ -343,11 +305,7 @@ extern "C" int b2v_ca_smoothing(float* vertices, int64_t nverts, const int64_t* 
   // adjacency: degrees, exclusive scan, fill
   k_mesh_degree<<<(unsigned)ceil_div64(nv + 1, 128), 128, 0, s>>>((const long long*)faces4, (const long long*)order, nv, w.first, w.last, w.deg);
   if ((rc = b2v_check_launch("k_mesh_degree"))) return rc;
-  const long long nb = ceil_div64(nv + 1, 2048);
-  k_scan_reduce<<<(unsigned)nb, 256, 0, s>>>(w.deg, nv + 1, w.bsum);
-  k_scan_bsums<<<1, 1, 0, s>>>(w.bsum, nb);
-  k_scan_apply<<<(unsigned)nb, 256, 0, s>>>(w.deg, nv + 1, w.bsum);
-  if ((rc = b2v_check_launch("k_scan"))) return rc;
+  if ((rc = scan(w.deg, nv + 1, w.bsum, nullptr, s))) return rc;
   k_mesh_adjacency<<<(unsigned)ceil_div64(nv, 128), 128, 0, s>>>((const long long*)faces4, (const long long*)order, nv, w.first, w.last, w.deg, w.adj);
   if ((rc = b2v_check_launch("k_mesh_adjacency"))) return rc;
   // seeds, then the frontier rounds of propagate_weights

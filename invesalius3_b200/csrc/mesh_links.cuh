@@ -1,5 +1,5 @@
-// The point -> cell links of a triangle mesh (vtkCellLinks), and the device-wide scan and stable radix sort
-// they are built with. Shared by the surface tools that walk a mesh through its links (connectivity.cu,
+// The point -> cell links of a triangle mesh (vtkCellLinks), and the stable radix sort they are built with
+// (the scan is scan.cuh's). Shared by the surface tools that walk a mesh through its links (connectivity.cu,
 // smoothing.cu, fill_holes.cu); every name is in an anonymous namespace, so each translation unit has its own
 // copy.
 //
@@ -13,67 +13,12 @@
 // warp match), only over the bits the largest key needs.
 #pragma once
 #include "b2v_common.cuh"
+#include "scan.cuh"
 
 namespace {
 
 constexpr int kBlock = 256;
-constexpr int kScanItems = 4;                      // items per thread of the device-wide scan
-constexpr int kScanTile = kBlock * kScanItems;
-
-int64_t scan_blocks(int64_t n) { return ceil_div64(n > 0 ? n : 1, kScanTile); }
-
-// ---- device-wide exclusive scan of uint64 in place (tiles of kScanTile, then the tile sums) ----------------
-__global__ void __launch_bounds__(kBlock) k_scan_tiles(unsigned long long* a, int64_t n,
-                                                       unsigned long long* sums) {
-  __shared__ unsigned long long s_w[kBlock / 32];
-  const int64_t base = (int64_t)blockIdx.x * kScanTile + (int64_t)threadIdx.x * kScanItems;
-  unsigned long long v[kScanItems], s = 0;
-  for (int k = 0; k < kScanItems; ++k) {
-    v[k] = base + k < n ? a[base + k] : 0ull;
-    s += v[k];
-  }
-  unsigned long long tot;
-  unsigned long long ex = block_exscan<unsigned long long>(s, s_w, &tot);
-  for (int k = 0; k < kScanItems; ++k) {
-    if (base + k < n) a[base + k] = ex;
-    ex += v[k];
-  }
-  if (threadIdx.x == 0) sums[blockIdx.x] = tot;
-}
-
-__global__ void __launch_bounds__(1024) k_scan_sums(unsigned long long* a, int64_t nb, unsigned long long* total) {
-  __shared__ unsigned long long s_w[32];
-  unsigned long long carry = 0;
-  for (int64_t base = 0; base < nb; base += blockDim.x) {
-    const int64_t i = base + threadIdx.x;
-    const unsigned long long x = i < nb ? a[i] : 0ull;
-    unsigned long long tot;
-    const unsigned long long ex = block_exscan<unsigned long long>(x, s_w, &tot);
-    if (i < nb) a[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0 && total) *total = carry;
-}
-
-__global__ void __launch_bounds__(kBlock) k_scan_add(unsigned long long* a, int64_t n,
-                                                     const unsigned long long* __restrict__ sums) {
-  const unsigned long long add = sums[blockIdx.x];
-  const int64_t base = (int64_t)blockIdx.x * kScanTile;
-  for (int k = threadIdx.x; k < kScanTile; k += kBlock)
-    if (base + k < n) a[base + k] += add;
-}
-
-// scratch: scan_blocks(n) + 1 words; total (may be null): the sum of a[0, n), written on the device
-int scan(unsigned long long* a, int64_t n, unsigned long long* scratch, unsigned long long* total, cudaStream_t s) {
-  const int64_t nb = scan_blocks(n);
-  B2V_REQUIRE(nb <= 0x7fffffffLL, B2V_ERR_ARG, "scan too long");
-  k_scan_tiles<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
-  if (int rc = b2v_check_launch("k_scan_tiles")) return rc;
-  k_scan_sums<<<1, 1024, 0, s>>>(scratch, nb, total);
-  if (int rc = b2v_check_launch("k_scan_sums")) return rc;
-  k_scan_add<<<(unsigned)nb, kBlock, 0, s>>>(a, n, scratch);
-  return b2v_check_launch("k_scan_add");
-}
+constexpr int kMaxBlocksPerSm = 2;                 // blocks per SM of a cooperative launch, at most
 
 // ---- stable LSD radix sort of (key, value) pairs, 8 bits a pass -------------------------------------------
 __global__ void __launch_bounds__(kBlock) k_rs_hist(const uint32_t* __restrict__ keys, int64_t n, int shift,
@@ -198,6 +143,17 @@ int build_links(W& w, const Faces& F, const char* what, cudaStream_t s) {
   if (int rc = sort_pairs(w, C3, bits_for(nv - 1), &lv, s)) return rc;
   k_copy_i32<<<b2v_grid(C3, kBlock, 16), kBlock, 0, s>>>(lv, C3, w.links);
   return b2v_check_launch("k_copy_i32");
+}
+
+// A cooperative launch of fn with kBlock threads and as many blocks as fit at once, at most kMaxBlocksPerSm
+// per SM. A kernel that does not fit is B2V_ERR_CUDA, reported as "<op>: <what> does not fit on an SM".
+inline int launch_coop(const void* fn, void** args, cudaStream_t s, const char* op, const char* what) {
+  int per_sm = 0;
+  B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlock, 0));
+  B2V_REQUIRE(per_sm >= 1, B2V_ERR_CUDA, "%s: %s does not fit on an SM", op, what);
+  if (per_sm > kMaxBlocksPerSm) per_sm = kMaxBlocksPerSm;
+  B2V_CUDA(cudaLaunchCooperativeKernel(fn, dim3(per_sm * b2v_sm_count()), dim3(kBlock), args, 0, s));
+  return b2v_check_launch(what);
 }
 
 }  // namespace

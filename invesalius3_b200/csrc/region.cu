@@ -6,7 +6,8 @@
 //   masked moments  count, min, max, np.mean and np.std of image[selection], bit-identical to NumPy. The
 //                   selection is `sel == value` or `sel > 127`, OR a clipped voxel box. Steps:
 //                     k_sel_count   per-tile selected counts (a tile is 4096 voxels, 16 per thread)
-//                     k_scan_tiles  exclusive scan of the tile counts -> tile offsets; the total goes to the host
+//                     k_scan_sums   exclusive scan of the tile counts in place -> tile offsets; the total goes
+//                                   to the host
 //                     k_compact<T>  the selected voxels in raveled order, in the image's dtype
 //                     k_pairwise    NumPy's pairwise summation (loops_utils.h.src) over subtrees of at most
 //                                   kSub elements, one block each; min and max ride along in the first pass
@@ -18,6 +19,7 @@
 #include <vector>
 
 #include "b2v_common.cuh"
+#include "scan.cuh"
 
 namespace {
 
@@ -86,78 +88,12 @@ __device__ __forceinline__ uint32_t sel_bits(const uint8_t* __restrict__ sel, co
   return bits;
 }
 
-// inclusive scan of v over the block (kThreads); `total` gets the block's sum
-__device__ __forceinline__ int block_scan(int v, int* s_warp, int& total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  constexpr int nw = kThreads / 32;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  if (lane == 31) s_warp[w] = v;
-  __syncthreads();
-  if (w == 0) {
-    int x = lane < nw ? s_warp[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < nw; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, x, o);
-      if (lane >= o) x += t;
-    }
-    if (lane < nw) s_warp[lane] = x;
-  }
-  __syncthreads();
-  if (w > 0) v += s_warp[w - 1];
-  total = s_warp[nw - 1];
-  __syncthreads();
-  return v;
-}
-
 __global__ void __launch_bounds__(kThreads) k_sel_count(const uint8_t* __restrict__ sel, const SelParams P,
-                                                        int32_t* __restrict__ counts) {
+                                                        long long* __restrict__ counts) {
   __shared__ int s_warp[kThreads / 32];
   const uint32_t bits = sel_bits(sel, P, (int64_t)blockIdx.x * kTile + (int64_t)threadIdx.x * kPer);
-  int total;
-  block_scan(__popc(bits), s_warp, total);
+  const int total = block_sum(__popc(bits), s_warp);
   if (threadIdx.x == 0) counts[blockIdx.x] = total;
-}
-
-// one block: offsets[t] = sum of counts[0..t), offsets[nt] = the total
-__global__ void __launch_bounds__(1024) k_scan_tiles(const int32_t* __restrict__ counts, int64_t nt,
-                                                     int64_t* __restrict__ offsets) {
-  __shared__ long long s_warp[32];
-  __shared__ long long s_carry;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (int64_t base = 0; base < nt; base += 1024) {
-    const int64_t t = base + threadIdx.x;
-    const long long c = t < nt ? counts[t] : 0;
-    long long v = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long u = __shfl_up_sync(0xffffffffu, v, o);
-      if (lane >= o) v += u;
-    }
-    if (lane == 31) s_warp[w] = v;
-    __syncthreads();
-    if (w == 0) {
-      long long x = s_warp[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const long long u = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += u;
-      }
-      s_warp[lane] = x;
-    }
-    __syncthreads();
-    const long long incl = v + (w > 0 ? s_warp[w - 1] : 0) + s_carry;
-    if (t < nt) offsets[t] = incl - c;
-    __syncthreads();
-    if (threadIdx.x == 1023) s_carry = incl;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[nt] = s_carry;
 }
 
 template <typename T>
@@ -167,10 +103,8 @@ __global__ void __launch_bounds__(kThreads) k_compact(const T* __restrict__ img,
   __shared__ int s_warp[kThreads / 32];
   const int64_t i0 = (int64_t)blockIdx.x * kTile + (int64_t)threadIdx.x * kPer;
   uint32_t bits = sel_bits(sel, P, i0);
-  const int c = __popc(bits);
   int total;
-  const int incl = block_scan(c, s_warp, total);
-  int64_t dst = offsets[blockIdx.x] + incl - c;
+  int64_t dst = offsets[blockIdx.x] + block_exscan<int, kThreads / 32>(__popc(bits), s_warp, &total);
   while (bits) {
     const int k = __ffs(bits) - 1;
     bits &= bits - 1;
@@ -216,7 +150,7 @@ __global__ void __launch_bounds__(kThreads) k_pairwise(const T* __restrict__ val
     const int L = tid < cnt ? s_len[d][tid] : 0;
     const int k = tid < cnt ? (L > 128 ? 2 : 1) : 0;
     int total;
-    const int first = block_scan(k, s_warp, total) - k;
+    const int first = block_exscan<int, kThreads / 32>(k, s_warp, &total);
     if (total == cnt) break;                       // uniform: nothing split, level d holds the leaves
     if (tid < cnt) {
       const int off = s_off[d & 1][tid];
@@ -309,12 +243,11 @@ double pw_combine(int64_t n, const double* part, size_t* idx) {
 
 int64_t max_subtrees(int64_t n) { return n / (kSub / 4) + 2; }   // every subtree of a split holds > kSub/2 - 8
 
-struct MomentsLayout { int64_t counts, offsets, vals, subs, part, total; };
+struct MomentsLayout { int64_t offsets, vals, subs, part, total; };
 MomentsLayout moments_layout(int64_t n) {
   const int64_t nt = ceil_div64(n, kTile), ms = max_subtrees(n);
   MomentsLayout L;
-  L.counts = 0;
-  L.offsets = align256(L.counts + nt * 4);
+  L.offsets = 0;
   L.vals = align256(L.offsets + (nt + 1) * 8);
   L.subs = align256(L.vals + n * 8);
   L.part = align256(L.subs + ms * 16);
@@ -422,11 +355,12 @@ extern "C" int b2v_masked_moments(const void* img, int dtype, int64_t dz, int64_
   cudaStream_t s = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   const MomentsLayout L = moments_layout(P.n);
-  k_sel_count<<<(unsigned)nt, kThreads, 0, s>>>(sel, P, (int32_t*)(ws + L.counts));
+  long long* offsets = (long long*)(ws + L.offsets);
+  k_sel_count<<<(unsigned)nt, kThreads, 0, s>>>(sel, P, offsets);
   int rc = b2v_check_launch("k_sel_count");
   if (rc) return rc;
-  k_scan_tiles<<<1, 1024, 0, s>>>((const int32_t*)(ws + L.counts), nt, (int64_t*)(ws + L.offsets));
-  if ((rc = b2v_check_launch("k_scan_tiles"))) return rc;
+  k_scan_sums<long long><<<1, 1024, 0, s>>>(offsets, nt, offsets + nt);
+  if ((rc = b2v_check_launch("k_scan_sums"))) return rc;
   int64_t count = 0;
   B2V_CUDA(cudaMemcpyAsync(&count, ws + L.offsets + nt * 8, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));

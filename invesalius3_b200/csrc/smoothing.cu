@@ -36,7 +36,6 @@ namespace cg = cooperative_groups;
 
 namespace {
 
-constexpr int kMaxBlocksPerSm = 2;
 constexpr int64_t kSmallLevels = 2048;             // peeling rounds this small run in one block
 constexpr int64_t kSmallSweep = 512;               // sweep levels this small run in one block
 enum : uint8_t { SIMPLE = 0, FIXED = 1, FEATURE = 2, BOUNDARY = 3, SKIPPED = 255 };   // VTK's vertex codes
@@ -395,15 +394,6 @@ __global__ void __launch_bounds__(kBlock, kMaxBlocksPerSm) k_sm_sweep(Sw S) {
   if (gtid() == 0) { S.ctl[C_ITERS] = t; S.ctl[C_SBAR] = bars; }
 }
 
-int launch_coop(const void* fn, void** args, cudaStream_t s, const char* what) {
-  int per_sm = 0;
-  B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlock, 0));
-  B2V_REQUIRE(per_sm >= 1, B2V_ERR_CUDA, "smoothing: %s does not fit on an SM", what);
-  if (per_sm > kMaxBlocksPerSm) per_sm = kMaxBlocksPerSm;
-  B2V_CUDA(cudaLaunchCooperativeKernel(fn, dim3(per_sm * b2v_sm_count()), dim3(kBlock), args, 0, s));
-  return b2v_check_launch(what);
-}
-
 int check_sizes(int64_t nv, int64_t nt, const char* what) {
   B2V_REQUIRE(nv >= 0 && nv <= 0x7fffffffLL && nt >= 0 && nt <= 0x7fffffffLL / 3, B2V_ERR_ARG,
               "%s: need V < 2^31 and 6T < 2^32", what);
@@ -484,7 +474,7 @@ extern "C" int b2v_smooth_analyse(const float* verts, int64_t nv, const void* fa
   if (int rc = b2v_check_launch("k_sm_roots")) return rc;
   Pk K{w.sstart, w.succ, w.indeg, w.order, w.loff, w.lcnt, (unsigned long long*)w.ctl};
   void* args[] = {&K};
-  if (int rc = launch_coop((const void*)k_sm_levels, args, s, "k_sm_levels")) return rc;
+  if (int rc = launch_coop((const void*)k_sm_levels, args, s, "smoothing", "k_sm_levels")) return rc;
 
   long long ctl[3];
   uint32_t b[6];
@@ -519,7 +509,7 @@ extern "C" int b2v_smooth_run(const float* verts, int64_t nv, int64_t nt, int64_
        relaxation, conv};
   B2V_CUDA(cudaMemsetAsync(w.ctl + C_MD, 0, (C_SBAR + 1 - C_MD) * 8, s));
   void* args[] = {&S};
-  if (int rc = launch_coop((const void*)k_sm_sweep, args, s, "k_sm_sweep")) return rc;
+  if (int rc = launch_coop((const void*)k_sm_sweep, args, s, "smoothing", "k_sm_sweep")) return rc;
   long long ctl[C_SBAR + 1];
   B2V_CUDA(cudaMemcpyAsync(ctl, w.ctl, sizeof(ctl), cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));

@@ -18,7 +18,7 @@
 //   k_vis_merge_insert exactly coincident vertices share one slot of an open-addressing hash table
 //                      (keys: the coordinate bits with -0 read as +0, compared with float ==).
 //   k_vis_first_use    atomicMin of the corner index over the kept faces, per slot.
-//   k_vis_block_counts / k_vis_scan_blocks / k_vis_emit_*   the O(T) compaction: a corner is the first
+//   k_vis_block_counts / k_scan_sums / k_vis_emit_*   the O(T) compaction: a corner is the first
 //                      use of its (merged) vertex when its index is that minimum; scans of those flags
 //                      number the output vertices, scans of the kept, non-degenerate faces order them.
 //
@@ -28,6 +28,7 @@
 #include <string.h>
 
 #include "b2v_common.cuh"
+#include "scan.cuh"
 
 namespace {
 
@@ -286,10 +287,6 @@ __global__ void __launch_bounds__(kBlock) k_vis_project(const float* __restrict_
   }
 }
 
-__global__ void __launch_bounds__(kBlock) k_vis_fill_u64(unsigned long long* p, int64_t n, unsigned long long v) {
-  for (int64_t i = gtid(); i < n; i += gstride()) p[i] = v;
-}
-
 // ---- rasterisation ----------------------------------------------------------------------------------------
 struct Tri {
   P3 a, b, c;
@@ -488,25 +485,6 @@ __global__ void __launch_bounds__(kBlock) k_vis_block_counts(Faces F, const uint
   }
 }
 
-// one block: exclusive scan of the per-block counts in place, totals to totals[0..1]
-__global__ void __launch_bounds__(1024) k_vis_scan_blocks(unsigned long long* bcount, int64_t nb,
-                                                          unsigned long long* totals) {
-  __shared__ unsigned long long s_w[32];
-  for (int part = 0; part < 2; ++part) {
-    unsigned long long* a = bcount + part * nb;
-    unsigned long long carry = 0;
-    for (int64_t base = 0; base < nb; base += blockDim.x) {
-      const int64_t i = base + threadIdx.x;
-      const unsigned long long x = i < nb ? a[i] : 0ull;
-      unsigned long long tot;
-      const unsigned long long ex = block_exscan<unsigned long long>(x, s_w, &tot);
-      if (i < nb) a[i] = carry + ex;
-      carry += tot;
-    }
-    if (threadIdx.x == 0) totals[part] = carry;
-  }
-}
-
 __global__ void __launch_bounds__(kBlock) k_vis_emit_verts(Faces F, const float* __restrict__ verts,
                                                            const uint8_t* __restrict__ vis, uint8_t flip,
                                                            const uint32_t* __restrict__ rep,
@@ -648,9 +626,9 @@ extern "C" int b2v_visibility_count(const float* verts, int64_t nv, const void* 
   B2V_CUDA(cudaMemsetAsync(w.slots, 0xff, (w.hmask + 1) * 4, s));
   B2V_CUDA(cudaMemsetAsync(w.first, 0xff, (w.hmask + 1) * 8, s));
 
-  k_vis_fill_u64<<<b2v_grid((int64_t)nviews * kPix, kBlock, 8), kBlock, 0, s>>>(w.zbuf, (int64_t)nviews * kPix,
-                                                                                kDepthOne);
-  if (int rc = b2v_check_launch("k_vis_fill_u64")) return rc;
+  k_fill<unsigned long long><<<b2v_grid((int64_t)nviews * kPix, kBlock, 8), kBlock, 0, s>>>(
+      w.zbuf, (int64_t)nviews * kPix, kDepthOne);
+  if (int rc = b2v_check_launch("k_fill")) return rc;
   k_vis_project<<<b2v_grid((int64_t)nviews * nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, nviews, w.cams, w.proj);
   if (int rc = b2v_check_launch("k_vis_project")) return rc;
   k_vis_merge_insert<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, w.hmask, w.slots, w.rep);
@@ -670,8 +648,8 @@ extern "C" int b2v_visibility_count(const float* verts, int64_t nv, const void* 
     B2V_REQUIRE(w.nb <= 0x7fffffffLL, B2V_ERR_ARG, "visibility_count: too many faces");
     k_vis_block_counts<<<(unsigned)w.nb, kBlock, 0, s>>>(F, w.vis, flip, w.rep, w.first, w.bcount, w.nb);
     if (int rc = b2v_check_launch("k_vis_block_counts")) return rc;
-    k_vis_scan_blocks<<<1, 1024, 0, s>>>(w.bcount, w.nb, w.totals);
-    if (int rc = b2v_check_launch("k_vis_scan_blocks")) return rc;
+    k_scan_sums<unsigned long long><<<2, 1024, 0, s>>>(w.bcount, w.nb, w.totals);
+    if (int rc = b2v_check_launch("k_scan_sums")) return rc;
   }
   unsigned long long tot[2];
   uint32_t status = 0;

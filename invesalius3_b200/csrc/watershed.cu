@@ -466,15 +466,7 @@ int ws_strct_bits(const uint8_t* st, int64_t odz, int64_t ody, int64_t odx, uint
   B2V_REQUIRE(st && odz >= 1 && ody >= 1 && odx >= 1 && odz <= 3 && ody <= 3 && odx <= 3 && (odz & 1) && (ody & 1) &&
                   (odx & 1),
               B2V_ERR_ARG, "watershed: the structuring element must be 1 or 3 wide on every axis");
-  uint32_t bits = 0;
-  for (int64_t kk = 0; kk < odz; ++kk)
-    for (int64_t jj = 0; jj < ody; ++jj)
-      for (int64_t ii = 0; ii < odx; ++ii)
-        if (st[(kk * ody + jj) * odx + ii]) {
-          int oz = (int)(kk - odz / 2), oy = (int)(jj - ody / 2), ox = (int)(ii - odx / 2);
-          if (oz || oy || ox) bits |= 1u << ((oz + 1) * 9 + (oy + 1) * 3 + (ox + 1));
-        }
-  *sb = bits;
+  *sb = strct_mask(st, odz, ody, odx) & ~(1u << 13);   // without the centre
   return B2V_OK;
 }
 
@@ -552,9 +544,8 @@ extern "C" int b2v_ws_flood(const uint16_t* img, const int16_t* markers, int64_t
     // 6-connected (the InVesalius default, generate_binary_structure(3, 1)): the persistent engine.
     // Offsets along an axis of extent 1 never apply, so they do not count.
     const uint32_t zb = (1u << 4) | (1u << 22), yb = (1u << 10) | (1u << 16), xb = (1u << 12) | (1u << 14);
-    const uint32_t six = zb | yb | xb;
     uint32_t eff = sb | (nz == 1 ? zb : 0u) | (ny == 1 ? yb : 0u) | (nx == 1 ? xb : 0u);
-    if (eff == six && !getenv("B2V_WS_GENERIC")) {
+    if (eff == kSB6 && !getenv("B2V_WS_GENERIC")) {
       int rounds = 0;
       rc = b2v_wsf_run(31, img, markers, nz, ny, nx, mode, 0, 0, labels, ambiguous, ambiguous ? 1 : 0, workspace, stream,
                        &rounds, 1);
