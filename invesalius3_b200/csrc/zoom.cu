@@ -12,19 +12,18 @@
 //                            float64 workspace; the y pass works in place.
 //     k_prefilter_rows       x axis: one warp per 32 rows. Rows move through shared memory in 32 x 16 tiles (two rows
 //                            of 128 bytes per load), each lane walks its row inside the tile.
-//   k_zoom_gather<T, ORDER>  one thread per output voxel: coordinate o * step per axis, B-spline weights, taps folded
-//                            by mirror, sum over the (ORDER + 1)^rank taps in row-major order, each value multiplied
-//                            by the axis weights in axis order. In 'constant' mode a coordinate past n - 1 (the last
-//                            sample's o * step can round just above it) writes cval, as SciPy does. Integer outputs
-//                            round half away from zero and clip to the type's range.
+//   k_resample<T, ORDER>     one thread per output voxel, one output slice per grid row: coordinate o * step - off
+//                            per axis, B-spline weights, taps folded by mirror, sum over the (ORDER + 1)^rank taps in
+//                            row-major order, each value multiplied by the axis weights in axis order. SciPy's 3-D
+//                            sum for volumes, its 2-D sum for a stack of slices, each slice with its own optional
+//                            (y, x) offset. 'constant' mode writes cval at a coordinate outside [0, n - 1] (the
+//                            last zoom sample's o * step can round just above n - 1), as SciPy does. Integer
+//                            outputs round half away from zero and clip to the type's range.
 //
 // scipy.ndimage.shift(input, shift, output, order <= 3, mode) with prefilter=True shares SciPy's routine with zoom
-// (zoom_shift): the same prefilter, weights, folding, tap order and rounding, with coordinate o - shift per axis.
-// Shift coordinates can be negative, so 'constant' mode writes cval on both sides (cc < 0 or cc > n - 1) and
-// 'mirror' folds negative coordinates as SciPy's map_coordinate does. Zoom coordinates are never negative, so
-// those branches leave zoom results unchanged.
-//   k_shift_gather<T, ORDER> one thread per output voxel, one slice per grid row: SciPy's 3-D sum for volumes, its
-//                            2-D sum for a stack of slices, each slice with its own (y, x) shift.
+// (zoom_shift): the same prefilter and the same gather, with coordinate o - shift per axis (step 1, off = shift)
+// where zoom has o * step (off 0). Shift coordinates can be negative, so 'mirror' folds negative coordinates as
+// SciPy's map_coordinate does; zoom coordinates never are, so that branch leaves zoom results unchanged.
 //
 // imagedata_utils.FixGantryTilt (imagedata_utils.py:143-154) shifts slice n of an int16 volume in place along y at
 // order 3 with cval = matrix.min() of the partly shifted volume. b2v_gantry_tilt evaluates it without the
@@ -34,7 +33,7 @@
 // gives the cvals, then the out-of-range outputs are filled.
 //   k_slice_min_i16          per-slice minimum of the original volume, before any slice is overwritten
 //   (prefilter, slab by slab) y then x passes over a slab of slices into a float64 workspace of the slab's size
-//   k_shift_gather<double,3> writes the in-range outputs in place, records per-slice in-range minima (warp
+//   k_resample<double, 3>    writes the in-range outputs in place, records per-slice in-range minima (warp
 //                            min-reduce, one int atomicMin per warp: order-independent) and out-of-range flags
 //   k_tilt_cval_chain        the scan over nz scalars (one thread)
 //   k_tilt_fill              writes each slice's cval into its out-of-range outputs
@@ -194,15 +193,24 @@ __global__ void __launch_bounds__(32 * kRowWarps) k_prefilter_rows(double* c, in
 }
 
 // ---- gather ---------------------------------------------------------------------------------------
+// Output index o of an axis samples input coordinate o * step - off. Zoom sets off = 0 and step = (n_in - 1) /
+// (n_out - 1); shift sets step = 1, off = shift and n_out = n_in. Both are exact in float64, so each keeps SciPy's
+// coordinate bit for bit: x - 0.0 == x (+0 included), o * 1.0 == o, and the library builds with -fmad=false, so
+// the multiply and the subtract are never fused.
 struct Axis {
   int64_t n_in, n_out;
-  double step;   // (n_in - 1) / (n_out - 1), or 1 when n_out == 1
+  double step, off;
 };
 
-struct GatherParams {
-  Axis ax[3];    // z, y, x; a 2-D zoom leaves the z axis unused
+struct ResampleParams {
+  Axis ax[3];                // z, y, x; a stack of 2-D slices when rank3 is 0 (a 2-D zoom: one slice)
+  const double* slice_off;   // stack of slices: per-slice (y, x) offsets on the device, or null (ax[1].off, ax[2].off)
   int rank3, mirror, out_dtype;
   double cval;
+  // Stack of slices with int16 output (gantry tilt): out-of-range outputs are left unwritten; slice_min receives
+  // the per-slice minimum of the in-range outputs and slice_out is set where a slice has an out-of-range output.
+  int* slice_min;
+  int* slice_out;
 };
 
 __device__ __forceinline__ int64_t fold_mirror(int64_t i, int64_t n) {
@@ -258,10 +266,10 @@ __device__ __forceinline__ bool taps_at(double cc, int64_t n_in, bool mirror, do
   return true;
 }
 
-// Coordinate, weights and folded tap indices of output index o along one zoomed axis
+// Weights and folded tap indices of output index o along one axis, at offset off
 template <int ORDER>
-__device__ __forceinline__ bool axis_taps(const Axis& A, int64_t o, bool mirror, double* w, int64_t* idx) {
-  return taps_at<ORDER>((double)o * A.step, A.n_in, mirror, w, idx);
+__device__ __forceinline__ bool axis_taps(const Axis& A, int64_t o, double off, bool mirror, double* w, int64_t* idx) {
+  return taps_at<ORDER>((double)o * A.step - off, A.n_in, mirror, w, idx);
 }
 
 template <typename T>
@@ -284,91 +292,39 @@ __device__ __forceinline__ void store_out(int out_dtype, void* out, int64_t i, d
   }
 }
 
+// Orders 0 and 1 are held to four blocks per SM (64 registers), which ptxas's own choice reaches only by spilling;
+// a minimum of 0 leaves orders 2 and 3 to ptxas.
 template <typename T, int ORDER>
-__global__ void __launch_bounds__(256) k_zoom_gather(const T* __restrict__ src, GatherParams P, void* out) {
+__global__ void __launch_bounds__(256, ORDER < 2 ? 4 : 0) k_resample(const T* __restrict__ src, ResampleParams P,
+                                                                    void* out) {
   const Axis &AZ = P.ax[0], &AY = P.ax[1], &AX = P.ax[2];
-  const int64_t total = AZ.n_out * AY.n_out * AX.n_out;
+  const int64_t in_area = AY.n_in * AX.n_in, area = AY.n_out * AX.n_out;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int kz_taps = P.rank3 ? ORDER + 1 : 1;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int64_t ox = i % AX.n_out, r = i / AX.n_out, oy = r % AY.n_out, oz = r / AY.n_out;
-    double wz[ORDER + 1], wy[ORDER + 1], wx[ORDER + 1];
-    int64_t iz[ORDER + 1], iy[ORDER + 1], ix[ORDER + 1];
-    bool inside = axis_taps<ORDER>(AY, oy, P.mirror, wy, iy) && axis_taps<ORDER>(AX, ox, P.mirror, wx, ix);
-    if (P.rank3) {
-      inside = axis_taps<ORDER>(AZ, oz, P.mirror, wz, iz) && inside;
-    } else {
-      iz[0] = 0;
-    }
-    double t = P.cval;
-    if (inside) {
-      t = 0.0;
-#pragma unroll
-      for (int a = 0; a <= ORDER; ++a) {
-        if (a == kz_taps) break;
-        const T* pz = src + iz[a] * AY.n_in * AX.n_in;
-#pragma unroll
-        for (int b = 0; b <= ORDER; ++b) {
-          const T* py = pz + iy[b] * AX.n_in;
-#pragma unroll
-          for (int c = 0; c <= ORDER; ++c) {
-            double v = to_f64(py[ix[c]]);
-            if (ORDER > 0) {
-              if (P.rank3) v *= wz[a];
-              v *= wy[b];
-              v *= wx[c];
-            }
-            t += v;
-          }
-        }
-      }
-    }
-    store_out(P.out_dtype, out, i, t);
-  }
-}
-
-// ---- shift --------------------------------------------------------------------------------------------
-struct ShiftParams {
-  int64_t nz, ny, nx;          // input = output shape; a stack of 2-D slices when rank3 is 0
-  double shift[3];             // z, y, x: output index o samples input coordinate o - shift
-  const double* slice_shift;   // stack of slices: per-slice (y, x) shifts on the device, or null (shift[1], shift[2])
-  int rank3, mirror, out_dtype;
-  double cval;
-  // Stack of slices with int16 output (gantry tilt): out-of-range outputs are left unwritten; slice_min receives
-  // the per-slice minimum of the in-range outputs and slice_out is set where a slice has an out-of-range output.
-  int* slice_min;
-  int* slice_out;
-};
-
-template <typename T, int ORDER>
-__global__ void __launch_bounds__(256) k_shift_gather(const T* __restrict__ src, ShiftParams P, void* out) {
-  const int64_t area = P.ny * P.nx;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int kz_taps = P.rank3 ? ORDER + 1 : 1;
-  for (int64_t oz = blockIdx.y; oz < P.nz; oz += gridDim.y) {   // uniform across the block
+  for (int64_t oz = blockIdx.y; oz < AZ.n_out; oz += gridDim.y) {   // uniform across the block
     double wz[ORDER + 1];
     int64_t iz[ORDER + 1];
     bool z_inside = true;
-    double sy = P.shift[1], sx = P.shift[2];
+    double offy = AY.off, offx = AX.off;
     const T* plane = src;
     iz[0] = 0;
     if (P.rank3) {
-      z_inside = taps_at<ORDER>((double)oz - P.shift[0], P.nz, P.mirror, wz, iz);
+      z_inside = axis_taps<ORDER>(AZ, oz, AZ.off, P.mirror, wz, iz);
     } else {
-      plane = src + oz * area;
-      if (P.slice_shift) {
-        sy = P.slice_shift[2 * oz];
-        sx = P.slice_shift[2 * oz + 1];
+      plane = src + oz * in_area;
+      if (P.slice_off) {
+        offy = P.slice_off[2 * oz];
+        offx = P.slice_off[2 * oz + 1];
       }
     }
     int vmin = INT_MAX;
     bool any_out = false;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < area; i += stride) {
-      const int64_t ox = i % P.nx, oy = i / P.nx, o = oz * area + i;
+      const int64_t ox = i % AX.n_out, oy = i / AX.n_out, o = oz * area + i;
       double wy[ORDER + 1], wx[ORDER + 1];
       int64_t iy[ORDER + 1], ix[ORDER + 1];
-      const bool inside = z_inside && taps_at<ORDER>((double)oy - sy, P.ny, P.mirror, wy, iy) &&
-                          taps_at<ORDER>((double)ox - sx, P.nx, P.mirror, wx, ix);
+      const bool inside = z_inside && axis_taps<ORDER>(AY, oy, offy, P.mirror, wy, iy) &&
+                          axis_taps<ORDER>(AX, ox, offx, P.mirror, wx, ix);
       if (!inside) {
         if (P.slice_min) any_out = true;
         else store_out(P.out_dtype, out, o, P.cval);
@@ -378,10 +334,10 @@ __global__ void __launch_bounds__(256) k_shift_gather(const T* __restrict__ src,
 #pragma unroll
       for (int a = 0; a <= ORDER; ++a) {
         if (a == kz_taps) break;
-        const T* pz = plane + iz[a] * area;
+        const T* pz = plane + iz[a] * in_area;
 #pragma unroll
         for (int b = 0; b <= ORDER; ++b) {
-          const T* py = pz + iy[b] * P.nx;
+          const T* py = pz + iy[b] * AX.n_in;
 #pragma unroll
           for (int c = 0; c <= ORDER; ++c) {
             double v = to_f64(py[ix[c]]);
@@ -518,36 +474,42 @@ int prefilter_volume(const void* in, int in_dtype, int64_t nz, int64_t ny, int64
   return prefilter_rows(ws, nx, nz * ny, order, s);
 }
 
+// One grid row per output slice, and across the rows about as many blocks as a grid-stride launch over every
+// output takes: a thread then loops over several outputs of its slice, which spreads its set-up over them.
 template <typename T, int ORDER>
-int gather_launch(const void* src, const GatherParams& P, void* out, cudaStream_t s) {
-  const int64_t total = P.ax[0].n_out * P.ax[1].n_out * P.ax[2].n_out;
-  k_zoom_gather<T, ORDER><<<b2v_grid(total, 256, 16), 256, 0, s>>>((const T*)src, P, out);
-  return b2v_check_launch("k_zoom_gather");
+int resample_launch(const void* src, const ResampleParams& P, void* out, cudaStream_t s) {
+  const int64_t nz = P.ax[0].n_out, rows = std::min<int64_t>(nz, 65535);
+  const int blocks = b2v_grid(nz * P.ax[1].n_out * P.ax[2].n_out, 256, 64);
+  k_resample<T, ORDER><<<dim3((unsigned)ceil_div64(blocks, rows), (unsigned)rows), 256, 0, s>>>((const T*)src, P, out);
+  return b2v_check_launch("k_resample");
 }
 
 // orders 2 and 3 gather from the float64 prefilter output only
 template <typename T>
-int gather_order(const void* src, int order, const GatherParams& P, void* out, cudaStream_t s) {
+int resample_order(const void* src, int order, const ResampleParams& P, void* out, cudaStream_t s) {
   if constexpr (std::is_same<T, double>::value) {
-    if (order == 2) return gather_launch<T, 2>(src, P, out, s);
-    if (order == 3) return gather_launch<T, 3>(src, P, out, s);
+    if (order == 2) return resample_launch<T, 2>(src, P, out, s);
+    if (order == 3) return resample_launch<T, 3>(src, P, out, s);
   }
-  return order == 0 ? gather_launch<T, 0>(src, P, out, s) : gather_launch<T, 1>(src, P, out, s);
+  return order == 0 ? resample_launch<T, 0>(src, P, out, s) : resample_launch<T, 1>(src, P, out, s);
 }
 
-template <typename T, int ORDER>
-int shift_launch(const void* src, const ShiftParams& P, void* out, cudaStream_t s) {
-  k_shift_gather<T, ORDER><<<slice_grid(P.nz, P.ny * P.nx), 256, 0, s>>>((const T*)src, P, out);
-  return b2v_check_launch("k_shift_gather");
-}
-
-template <typename T>
-int shift_order(const void* src, int order, const ShiftParams& P, void* out, cudaStream_t s) {
-  if constexpr (std::is_same<T, double>::value) {
-    if (order == 2) return shift_launch<T, 2>(src, P, out, s);
-    if (order == 3) return shift_launch<T, 3>(src, P, out, s);
+// zoom and shift once their arguments are checked and P's axes filled in: the prefilter into the workspace at
+// orders 2 and 3, then the gather from the input's dtype or from the float64 workspace
+int resample(const void* in, int in_dtype, int order, const ResampleParams& P, void* out, void* workspace,
+             cudaStream_t s) {
+  if (order >= 2) {
+    const int rc =
+        prefilter_volume(in, in_dtype, P.ax[0].n_in, P.ax[1].n_in, P.ax[2].n_in, order, (double*)workspace, s);
+    if (rc) return rc;
+    return resample_order<double>(workspace, order, P, out, s);
   }
-  return order == 0 ? shift_launch<T, 0>(src, P, out, s) : shift_launch<T, 1>(src, P, out, s);
+  switch (in_dtype) {
+    case B2V_I16: return resample_order<int16_t>(in, order, P, out, s);
+    case B2V_U8: return resample_order<uint8_t>(in, order, P, out, s);
+    case B2V_F32: return resample_order<float>(in, order, P, out, s);
+    default: return resample_order<double>(in, order, P, out, s);
+  }
 }
 
 constexpr int64_t kTiltSlabBytes = int64_t(1) << 30;   // default float64 workspace of the gantry-tilt slab
@@ -578,34 +540,18 @@ extern "C" int b2v_zoom(const void* in, int in_dtype, int ndim, int64_t nz, int6
   if (out_nz * out_ny * out_nx == 0) return B2V_OK;
   B2V_REQUIRE(in && out, B2V_ERR_ARG, "zoom: null pointer");
   B2V_REQUIRE(order < 2 || workspace, B2V_ERR_ARG, "zoom: orders 2 and 3 need the workspace");
-  cudaStream_t s = (cudaStream_t)stream;
 
-  const void* src = in;
-  int src_dtype = in_dtype;
-  if (order >= 2) {
-    const int rc = prefilter_volume(in, in_dtype, nz, ny, nx, order, (double*)workspace, s);
-    if (rc) return rc;
-    src = workspace;
-    src_dtype = B2V_F64;
-  }
-
-  GatherParams P;
+  ResampleParams P = {};
   const int64_t n_in[3] = {nz, ny, nx}, n_out[3] = {out_nz, out_ny, out_nx};
   for (int a = 0; a < 3; ++a) {
-    P.ax[a].n_in = n_in[a];
-    P.ax[a].n_out = n_out[a];
-    P.ax[a].step = n_out[a] > 1 ? (double)(n_in[a] - 1) / (double)(n_out[a] - 1) : 1.0;
+    const double step = n_out[a] > 1 ? (double)(n_in[a] - 1) / (double)(n_out[a] - 1) : 1.0;
+    P.ax[a] = {n_in[a], n_out[a], step, 0.0};
   }
   P.rank3 = ndim == 3;
   P.mirror = mode == B2V_ZOOM_MIRROR;
   P.out_dtype = out_dtype;
   P.cval = cval;
-  switch (src_dtype) {
-    case B2V_I16: return gather_order<int16_t>(src, order, P, out, s);
-    case B2V_U8: return gather_order<uint8_t>(src, order, P, out, s);
-    case B2V_F32: return gather_order<float>(src, order, P, out, s);
-    default: return gather_order<double>(src, order, P, out, s);
-  }
+  return resample(in, in_dtype, order, P, out, workspace, (cudaStream_t)stream);
 }
 
 extern "C" int64_t b2v_shift_workspace_bytes(int64_t nz, int64_t ny, int64_t nx, int order) {
@@ -626,34 +572,16 @@ extern "C" int b2v_shift(const void* in, int in_dtype, int ndim, int64_t nz, int
   B2V_REQUIRE(in && out && shift, B2V_ERR_ARG, "shift: null pointer");
   B2V_REQUIRE(in != out, B2V_ERR_ARG, "shift: the output must not be the input");
   B2V_REQUIRE(order < 2 || workspace, B2V_ERR_ARG, "shift: orders 2 and 3 need the workspace");
-  cudaStream_t s = (cudaStream_t)stream;
 
-  const void* src = in;
-  int src_dtype = in_dtype;
-  if (order >= 2) {
-    const int rc = prefilter_volume(in, in_dtype, nz, ny, nx, order, (double*)workspace, s);
-    if (rc) return rc;
-    src = workspace;
-    src_dtype = B2V_F64;
-  }
-
-  ShiftParams P = {};
-  P.nz = nz;
-  P.ny = ny;
-  P.nx = nx;
-  P.shift[0] = ndim == 3 ? shift[0] : 0.0;
-  P.shift[1] = shift[ndim - 2];
-  P.shift[2] = shift[ndim - 1];
+  ResampleParams P = {};
+  const int64_t n[3] = {nz, ny, nx};
+  const double off[3] = {ndim == 3 ? shift[0] : 0.0, shift[ndim - 2], shift[ndim - 1]};
+  for (int a = 0; a < 3; ++a) P.ax[a] = {n[a], n[a], 1.0, off[a]};
   P.rank3 = ndim == 3;
   P.mirror = mode == B2V_ZOOM_MIRROR;
   P.out_dtype = out_dtype;
   P.cval = cval;
-  switch (src_dtype) {
-    case B2V_I16: return shift_order<int16_t>(src, order, P, out, s);
-    case B2V_U8: return shift_order<uint8_t>(src, order, P, out, s);
-    case B2V_F32: return shift_order<float>(src, order, P, out, s);
-    default: return shift_order<double>(src, order, P, out, s);
-  }
+  return resample(in, in_dtype, order, P, out, workspace, (cudaStream_t)stream);
 }
 
 // workspace: [slab][ny][nx] float64 coefficients, nz (y, x) shifts, then four int arrays of nz
@@ -686,20 +614,20 @@ extern "C" int b2v_gantry_tilt(int16_t* vol, int64_t nz, int64_t ny, int64_t nx,
   k_slice_min_i16<<<slice_grid(nz, area), 256, 0, s>>>(vol, nz, area, orig_min);
   if ((rc = b2v_check_launch("k_slice_min_i16"))) return rc;
 
-  ShiftParams P = {};
-  P.ny = ny;
-  P.nx = nx;
+  ResampleParams P = {};
+  P.ax[1] = {ny, ny, 1.0, 0.0};
+  P.ax[2] = {nx, nx, 1.0, 0.0};
   P.out_dtype = B2V_I16;
   for (int64_t z0 = 0; z0 < nz; z0 += slab) {
     const int64_t n = std::min(slab, nz - z0);
     int16_t* sv = vol + z0 * area;   // the slab's slices are read by the prefilter before the gather overwrites them
     if ((rc = prefilter_first<int16_t>(sv, ws, ny, nx, n * nx, 3, s))) return rc;
     if ((rc = prefilter_rows(ws, nx, n * ny, 3, s))) return rc;
-    P.nz = n;
-    P.slice_shift = d_shift + 2 * z0;
+    P.ax[0] = {n, n, 1.0, 0.0};
+    P.slice_off = d_shift + 2 * z0;
     P.slice_min = inrange_min + z0;
     P.slice_out = slice_out + z0;
-    if ((rc = shift_launch<double, 3>(ws, P, sv, s))) return rc;
+    if ((rc = resample_launch<double, 3>(ws, P, sv, s))) return rc;
   }
   k_tilt_cval_chain<<<1, 32, 0, s>>>(nz, orig_min, inrange_min, slice_out, cval, cvals);
   if ((rc = b2v_check_launch("k_tilt_cval_chain"))) return rc;

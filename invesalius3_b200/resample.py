@@ -35,18 +35,46 @@ _NP = {np.dtype(np.int16): torch.int16, np.dtype(np.uint8): torch.uint8, np.dtyp
 _MODES = {"constant": _lib.ZOOM_CONSTANT, "mirror": _lib.ZOOM_MIRROR}
 
 
-def _factors(zoom, ndim: int) -> tuple[float, ...]:
-    if np.ndim(zoom) == 0:
-        return (float(zoom),) * ndim
-    z = tuple(float(f) for f in zoom)
-    if len(z) != ndim:
+def _per_axis(value, ndim: int) -> tuple[float, ...]:
+    """A zoom factor or shift: one number for every axis, or one per axis."""
+    if np.ndim(value) == 0:
+        return (float(value),) * ndim
+    v = tuple(float(x) for x in value)
+    if len(v) != ndim:
         raise RuntimeError("sequence argument must have length equal to input rank")   # SciPy's message
-    return z
+    return v
+
+
+def _check_built(name: str, t_dtype, out_dtype, ndim: int, order: int, mode: str) -> None:
+    if ndim not in (2, 3):
+        raise NotImplementedError(f"{name}: 2-D or 3-D input only")
+    if t_dtype not in _CODE or out_dtype not in _CODE:
+        raise NotImplementedError(f"{name}: dtypes int16, uint8, float32, float64 only ({t_dtype} -> {out_dtype})")
+    if order not in (0, 1, 2, 3):
+        raise NotImplementedError(f"{name}: spline order {order} not built (0-3)")
+    if mode not in _MODES:
+        raise NotImplementedError(f"{name}: mode {mode!r} not built ('constant', 'mirror')")
+
+
+def _output(name: str, output, dtype, shape) -> np.ndarray:
+    """The array that receives a result of `shape`: `output` itself if it is an array, else a new array of the
+    dtype `output` names (None: `dtype`, the input's)."""
+    if output is None:
+        out_dtype = dtype
+    elif isinstance(output, np.ndarray):
+        if output.shape != shape:
+            raise RuntimeError("output shape not correct")   # SciPy's message
+        out_dtype = output.dtype
+    else:
+        out_dtype = np.dtype(output)
+    if out_dtype not in _NP:
+        raise NotImplementedError(f"{name}: output dtype {out_dtype} is not built (int16, uint8, float32, float64)")
+    return output if isinstance(output, np.ndarray) else np.empty(shape, out_dtype)
 
 
 def output_shape(shape, zoom) -> tuple[int, ...]:
     """SciPy's output shape: round(n * factor) per axis (Python's round, ties to even)."""
-    return tuple(int(round(n * f)) for n, f in zip(shape, _factors(zoom, len(shape))))
+    return tuple(int(round(n * f)) for n, f in zip(shape, _per_axis(zoom, len(shape))))
 
 
 def zoom_device(t: torch.Tensor, zoom, order: int, out_dtype: torch.dtype, cval: float = 0.0,
@@ -55,15 +83,8 @@ def zoom_device(t: torch.Tensor, zoom, order: int, out_dtype: torch.dtype, cval:
     int16, uint8, float32 or float64; returns a new tensor of out_dtype. Where every factor is 1 the
     result is t cast to out_dtype, as SciPy returns its input unchanged."""
     _dense(t, "image")
-    if t.dim() not in (2, 3):
-        raise NotImplementedError("zoom_device: 2-D or 3-D input only")
-    if t.dtype not in _CODE or out_dtype not in _CODE:
-        raise NotImplementedError(f"zoom_device: dtypes int16, uint8, float32, float64 only ({t.dtype} -> {out_dtype})")
-    if order not in (0, 1, 2, 3):
-        raise NotImplementedError(f"zoom_device: spline order {order} not built (0-3)")
-    if mode not in _MODES:
-        raise NotImplementedError(f"zoom_device: mode {mode!r} not built ('constant', 'mirror')")
-    factors = _factors(zoom, t.dim())
+    _check_built("zoom_device", t.dtype, out_dtype, t.dim(), order, mode)
+    factors = _per_axis(zoom, t.dim())
     shape = output_shape(t.shape, factors)
     if all(f == 1 for f in factors):
         return t.to(out_dtype, copy=True)
@@ -92,49 +113,16 @@ def zoom(input, zoom, output=None, order: int = 3, mode: str = "constant", cval:
         raise NotImplementedError(f"zoom: dtype {a.dtype} is not built (int16, uint8, float32, float64)")
     if a.ndim not in (2, 3):
         raise NotImplementedError("zoom: 2-D or 3-D input only")
-    shape = output_shape(a.shape, zoom)
-    res = None
-    if output is None:
-        out_dtype = a.dtype
-    elif isinstance(output, np.ndarray):
-        if output.shape != shape:
-            raise RuntimeError("output shape not correct")   # SciPy's message
-        res, out_dtype = output, output.dtype
-    else:
-        out_dtype = np.dtype(output)
-    if out_dtype not in _NP:
-        raise NotImplementedError(f"zoom: output dtype {out_dtype} is not built (int16, uint8, float32, float64)")
-    if res is None:
-        res = np.empty(shape, out_dtype)
-    if all(f == 1 for f in _factors(zoom, a.ndim)):
+    res = _output("zoom", output, a.dtype, output_shape(a.shape, zoom))
+    if all(f == 1 for f in _per_axis(zoom, a.ndim)):
         res[...] = a
         return res
     if a.size == 0 or res.size == 0:
         return res
     t = dev.to_device(a)
-    o = zoom_device(t, zoom, order, _NP[out_dtype], cval, mode)
+    o = zoom_device(t, zoom, order, _NP[res.dtype], cval, mode)
     dev.to_host(o, res)
     return res
-
-
-def _shifts(shift, ndim: int) -> tuple[float, ...]:
-    if np.ndim(shift) == 0:
-        return (float(shift),) * ndim
-    s = tuple(float(v) for v in shift)
-    if len(s) != ndim:
-        raise RuntimeError("sequence argument must have length equal to input rank")   # SciPy's message
-    return s
-
-
-def _check_built(name: str, t_dtype, out_dtype, ndim: int, order: int, mode: str) -> None:
-    if ndim not in (2, 3):
-        raise NotImplementedError(f"{name}: 2-D or 3-D input only")
-    if t_dtype not in _CODE or out_dtype not in _CODE:
-        raise NotImplementedError(f"{name}: dtypes int16, uint8, float32, float64 only ({t_dtype} -> {out_dtype})")
-    if order not in (0, 1, 2, 3):
-        raise NotImplementedError(f"{name}: spline order {order} not built (0-3)")
-    if mode not in _MODES:
-        raise NotImplementedError(f"{name}: mode {mode!r} not built ('constant', 'mirror')")
 
 
 def shift_device(t: torch.Tensor, shift, order: int, out_dtype: torch.dtype, cval: float = 0.0,
@@ -143,7 +131,7 @@ def shift_device(t: torch.Tensor, shift, order: int, out_dtype: torch.dtype, cva
     int16, uint8, float32 or float64; returns a new tensor of out_dtype and t's shape."""
     _dense(t, "image")
     _check_built("shift_device", t.dtype, out_dtype, t.dim(), order, mode)
-    sh = (C.c_double * t.dim())(*_shifts(shift, t.dim()))
+    sh = (C.c_double * t.dim())(*_per_axis(shift, t.dim()))
     out = torch.empty(t.shape, dtype=out_dtype, device=t.device)
     if t.numel() == 0:
         return out
@@ -166,24 +154,12 @@ def shift(input, shift, output=None, order: int = 3, mode: str = "constant", cva
         raise NotImplementedError(f"shift: dtype {a.dtype} is not built (int16, uint8, float32, float64)")
     if a.ndim not in (2, 3):
         raise NotImplementedError("shift: 2-D or 3-D input only")
-    res = None
-    if output is None:
-        out_dtype = a.dtype
-    elif isinstance(output, np.ndarray):
-        if output.shape != a.shape:
-            raise RuntimeError("output shape not correct")   # SciPy's message
-        res, out_dtype = output, output.dtype
-    else:
-        out_dtype = np.dtype(output)
-    if out_dtype not in _NP:
-        raise NotImplementedError(f"shift: output dtype {out_dtype} is not built (int16, uint8, float32, float64)")
-    _check_built("shift", _NP[a.dtype], _NP[out_dtype], a.ndim, order, mode)
-    _shifts(shift, a.ndim)
-    if res is None:
-        res = np.empty(a.shape, out_dtype)
+    res = _output("shift", output, a.dtype, a.shape)
+    _check_built("shift", _NP[a.dtype], _NP[res.dtype], a.ndim, order, mode)
+    _per_axis(shift, a.ndim)
     if a.size == 0:
         return res
-    o = shift_device(dev.to_device(a), shift, order, _NP[out_dtype], cval, mode)
+    o = shift_device(dev.to_device(a), shift, order, _NP[res.dtype], cval, mode)
     dev.to_host(o, res)
     return res
 
