@@ -589,6 +589,33 @@ int b2v_holes_emit(const void* faces, int64_t nv, int64_t nt, int face_cols, int
                    const int64_t* counts_host, void* workspace, void* faces_out, int64_t* first_line,
                    int64_t* npts, double* radius, int8_t* status, void* stream);
 
+/* ---- surface normals, volume and area --------------------------------------------------------------------
+ * vtkPolyDataNormals on triangles with consistency, splitting and non-manifold traversal on, and
+ * vtkMassProperties' volume and area, behind every InVesalius surface (surface_process, surface.py,
+ * viewer_volume, brainmesh_handler). The contract is restated in the C checker, normals.c; the result equals
+ * the sequential filter bit for bit. verts float32 [nv][3]; faces int32 / int64 (faces_i64) [nt][face_cols],
+ * face_cols 3, or 4 with a leading 3. A bad face or a NaN feature angle is B2V_ERR_ARG; the angle (degrees)
+ * is clamped to [0, 180]. The workspace (b2v_normals_workspace_bytes) serves all three calls.
+ *   b2v_normals_count   orders, orients (auto_orient != 0: VTK's leftmost-point seeds), computes the cell
+ *                       normals and splits; synchronises. counts_host[4] = {regions, flips, new points,
+ *                       waves}.
+ *   b2v_normals_emit    from the same workspace: points_out float32 [nv + new][3], faces_out [nt][face_cols]
+ *                       in the input's dtype and form, point_normals float32 [nv + new][3], cell_normals
+ *                       float32 [nt][3]. Does not synchronise.
+ *   b2v_mass_properties out_host[2] = {volume, area} (doubles, on the host); synchronises.
+ *   b2v_normals_layout  byte offsets in the workspace: [0] uint8 [nt] 1 where a cell was reversed, [1] int32
+ *                       cells in wave order, [2] float64 [nt][4] the mass terms of each triangle (area, then
+ *                       the x, y, z projected-volume terms), [3] int8 [nt] its normal class. */
+int64_t b2v_normals_workspace_bytes(int64_t nv, int64_t nt);
+int b2v_normals_layout(int64_t nv, int64_t nt, int64_t* layout_out);
+int b2v_normals_count(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                      double feature_angle, int auto_orient, void* workspace, void* stream, int64_t* counts_host);
+int b2v_normals_emit(const float* verts, int64_t nv, int64_t nt, int face_cols, int faces_i64,
+                     const int64_t* counts_host, void* workspace, float* points_out, void* faces_out,
+                     float* point_normals, float* cell_normals, void* stream);
+int b2v_mass_properties(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
+                        void* workspace, void* stream, double* out_host);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

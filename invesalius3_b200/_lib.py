@@ -148,6 +148,11 @@ PROTOTYPES = {
     "b2v_holes_layout": (cint, [i64, i64, C.POINTER(i64)]),
     "b2v_holes_count": (cint, [vp, i64, vp, i64, cint, cint, dbl, vp, vp, C.POINTER(i64)]),
     "b2v_holes_emit": (cint, [vp, i64, i64, cint, cint, C.POINTER(i64), vp, vp, vp, vp, vp, vp, vp]),
+    "b2v_normals_workspace_bytes": (i64, [i64, i64]),
+    "b2v_normals_layout": (cint, [i64, i64, C.POINTER(i64)]),
+    "b2v_normals_count": (cint, [vp, i64, vp, i64, cint, cint, dbl, cint, vp, vp, C.POINTER(i64)]),
+    "b2v_normals_emit": (cint, [vp, i64, i64, cint, cint, C.POINTER(i64), vp, vp, vp, vp, vp, vp]),
+    "b2v_mass_properties": (cint, [vp, i64, vp, i64, cint, cint, vp, vp, C.POINTER(dbl)]),
 }
 
 VIS_CAMERA_DOUBLES = 32

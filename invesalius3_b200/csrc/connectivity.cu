@@ -10,31 +10,24 @@
 //   k_cc_*               union-find over the triangle-point incidence (hook, then compress); each
 //                        component's minimum cell; a scan of the "minimum cell" flags numbers the regions
 //                        and lists their first cells: wave 0 of every region at once.
-//   k_conn_levels        one persistent cooperative launch runs every wave of every region: the appended
-//                        list of wave L+1 is laid out by a scan over wave L (parent order, then j, then link
-//                        order), each unmarked candidate takes the atomicMin of its positions, and a second
-//                        scan compacts the winners in position order. That is VTK's processing order, in
-//                        linear work and without a sort. A wave of at most kSmall cells runs in block 0
-//                        alone, with block barriers, until the waves grow again.
+//   k_waves<ConnNb>      one persistent cooperative launch runs every wave of every region (waves.cuh): the
+//                        appended list of wave L+1 is laid out by a scan over wave L (parent order, then j,
+//                        then link order), each unmarked candidate takes the atomicMin of its positions, and
+//                        a second scan compacts the winners in position order. That is VTK's processing
+//                        order, in linear work and without a sort.
 //   sort by region       the processed sequence (wave-major) stably sorted by region: region-major ranks.
 //   k_conn_first_use     each point takes the atomicMin of (rank, j) over its corners; a scan of the
 //                        first-use flags is PointMap, region by region.
 //   faces                the visited cells, in ascending id, stably sorted by region.
 //
 // Stable sorts are the radix sort of mesh_links.cuh.
-#include <cooperative_groups.h>
 #include <string.h>
 
 #include "b2v_common.cuh"
 #include "mesh_links.cuh"
-
-namespace cg = cooperative_groups;
+#include "waves.cuh"
 
 namespace {
-
-constexpr int kMaxGrid = 1024;                     // blocks of the persistent launch (btot capacity)
-constexpr int64_t kSmall = 2048;                   // waves this small run in one block
-constexpr unsigned long long kInf = ~0ull;
 
 struct ConnWs {
   long long* ctl;                  // [0..15]: two state records for the persistent launch, then results
@@ -113,26 +106,7 @@ ConnWs carve(void* base, int64_t nv, int64_t nt, int64_t nseeds) {
   return w;
 }
 
-// ---- union-find partition --------------------------------------------------------------------------------
-__device__ __forceinline__ int32_t uf_find(const int32_t* parent, int32_t x) {
-  const volatile int32_t* p = parent;
-  int32_t y = p[x];
-  while (y != x) { x = y; y = p[x]; }
-  return x;
-}
-
-__device__ __forceinline__ void uf_unite(int32_t* parent, int32_t a, int32_t b) {
-  for (;;) {
-    a = uf_find(parent, a);
-    b = uf_find(parent, b);
-    if (a == b) return;
-    if (a > b) { const int32_t t = a; a = b; b = t; }
-    const int32_t old = atomicCAS(&parent[b], b, a);   // hook the larger root under the smaller
-    if (old == b) return;
-    b = old;
-  }
-}
-
+// ---- union-find partition (uf_find / uf_unite: mesh_links.cuh) ------------------------------------------
 __global__ void __launch_bounds__(kBlock) k_cc_init(int32_t* parent, uint32_t* cmin, int64_t nv) {
   for (int64_t p = gtid(); p < nv; p += gstride()) { parent[p] = (int32_t)p; cmin[p] = 0xffffffffu; }
 }
@@ -183,178 +157,45 @@ __global__ void __launch_bounds__(kBlock) k_conn_reset(int32_t* reg, unsigned lo
   for (int64_t t = gtid(); t < nt; t += gstride()) { reg[t] = -1; best[t] = kInf; }
 }
 
-// ---- the waves ---------------------------------------------------------------------------------------------
-struct Lv {
+// ---- the waves: TraverseAndMark's enumeration for waves.cuh -----------------------------------------------
+// An item is a cell of seq, or in the seed wave a seed point; its entries are the link lists of its points,
+// in point order j, then link order. A winner inherits the region of the item that claimed it.
+struct ConnNb {
   const int32_t* tri;
   const unsigned long long* lstart;
   const int32_t* links;
   const int64_t* seeds;
-  int32_t* seq;
+  const int32_t* seq;
   int32_t* reg;
-  unsigned long long* best;
-  unsigned long long* loc1;
-  unsigned long long* loc2;
-  unsigned long long* btot;    // [0, kMaxGrid): appended entries per block; [kMaxGrid, 2 kMaxGrid): winners
-};
 
-// one wave; every block of a team computes the same record from the per-block totals
-struct State {
-  long long n;        // cells (or seeds) of the current wave
-  long long cur;      // its offset in seq (the seed wave: none)
-  long long base;     // first position of the wave's appended list; every earlier position is smaller
-  long long depth;    // waves that marked a cell
-  long long total;    // cells marked so far
-  long long seed;     // 1 while the current wave is the list of seeds
-};
-
-__device__ __forceinline__ int item_points(const Lv& P, const State& st, int64_t i, int32_t pts[3]) {
-  if (st.seed) {
-    const int64_t s = P.seeds[i];
-    pts[0] = (int32_t)s;
-    return s >= 0 ? 1 : 0;
-  }
-  const int32_t c = P.seq[st.cur + i];
-  pts[0] = P.tri[3 * c]; pts[1] = P.tri[3 * c + 1]; pts[2] = P.tri[3 * c + 2];
-  return 3;
-}
-
-// sum over blocks [0, b) and [0, nb) of btot[off + .], with the block's threads; s_r: 2 shared words
-__device__ __forceinline__ void block_prefix(const unsigned long long* btot, int b, int nb,
-                                             unsigned long long* s_r) {
-  if (threadIdx.x < 32) {
-    unsigned long long pre = 0, all = 0;
-    for (int k = threadIdx.x; k < nb; k += 32) {
-      const unsigned long long x = ((const volatile unsigned long long*)btot)[k];
-      all += x;
-      if (k < b) pre += x;
+  __device__ __forceinline__ int points(const State& st, int64_t i, int32_t pts[3]) const {
+    if (st.seed) {
+      const int64_t s = seeds[i];
+      pts[0] = (int32_t)s;
+      return s >= 0 ? 1 : 0;
     }
-    for (int o = 16; o > 0; o >>= 1) {
-      pre += __shfl_xor_sync(0xffffffffu, pre, o);
-      all += __shfl_xor_sync(0xffffffffu, all, o);
-    }
-    if (threadIdx.x == 0) { s_r[0] = pre; s_r[1] = all; }
+    const int32_t c = seq[st.cur + i];
+    pts[0] = tri[3 * c]; pts[1] = tri[3 * c + 1]; pts[2] = tri[3 * c + 2];
+    return 3;
   }
-  __syncthreads();
-}
-
-template <bool kGrid>
-__device__ __forceinline__ void team_sync(cg::grid_group& g) {
-  if (kGrid) g.sync(); else __syncthreads();
-}
-
-template <bool kGrid>
-__device__ void run_wave(const Lv& P, State& st, int b, int nb, cg::grid_group& g) {
-  __shared__ unsigned long long s_w[kBlock / 32];
-  __shared__ unsigned long long s_r[4];
-  const int64_t chunk = ceil_div64(st.n, nb);
-  const int64_t lo = (int64_t)b * chunk, hi = lo + chunk < st.n ? lo + chunk : st.n;
-  // 1. entries each item appends: the link lengths of its points
-  unsigned long long carry = 0;
-  for (int64_t t0 = lo; t0 < hi; t0 += kBlock) {
-    const int64_t i = t0 + threadIdx.x;
-    unsigned long long c = 0;
-    if (i < hi) {
-      int32_t pts[3];
-      const int np = item_points(P, st, i, pts);
-      for (int j = 0; j < np; ++j) c += P.lstart[pts[j] + 1] - P.lstart[pts[j]];
-    }
-    unsigned long long tot;
-    const unsigned long long ex = block_exscan<unsigned long long>(c, s_w, &tot);
-    if (i < hi) P.loc1[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0) P.btot[b] = carry;
-  team_sync<kGrid>(g);
-  // 2. every unmarked candidate takes the lowest of its positions
-  block_prefix(P.btot, b, nb, s_r);
-  const unsigned long long pre1 = s_r[0] + (unsigned long long)st.base, all1 = s_r[1];
-  for (int64_t i = lo + threadIdx.x; i < hi; i += kBlock) {
-    unsigned long long q = pre1 + P.loc1[i];
+  __device__ __forceinline__ unsigned long long count(const State& st, int64_t i) const {
     int32_t pts[3];
-    const int np = item_points(P, st, i, pts);
-    for (int j = 0; j < np; ++j)
-      for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q) {
-        const int32_t d = P.links[k];
-        if (((volatile unsigned long long*)P.best)[d] >= (unsigned long long)st.base) atomicMin(&P.best[d], q);
-      }
-  }
-  team_sync<kGrid>(g);
-  // 3. winners per item: the entries at their cell's lowest position
-  carry = 0;
-  for (int64_t t0 = lo; t0 < hi; t0 += kBlock) {
-    const int64_t i = t0 + threadIdx.x;
+    const int np = points(st, i, pts);
     unsigned long long c = 0;
-    if (i < hi) {
-      unsigned long long q = pre1 + P.loc1[i];
-      int32_t pts[3];
-      const int np = item_points(P, st, i, pts);
-      for (int j = 0; j < np; ++j)
-        for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q)
-          c += P.best[P.links[k]] == q;
-    }
-    unsigned long long tot;
-    const unsigned long long ex = block_exscan<unsigned long long>(c, s_w, &tot);
-    if (i < hi) P.loc2[i] = carry + ex;
-    carry += tot;
+    for (int j = 0; j < np; ++j) c += lstart[pts[j] + 1] - lstart[pts[j]];
+    return c;
   }
-  if (threadIdx.x == 0) P.btot[kMaxGrid + b] = carry;
-  team_sync<kGrid>(g);
-  // 4. the winners, in position order, are the next wave; they inherit the parent's region
-  block_prefix(P.btot + kMaxGrid, b, nb, s_r + 2);
-  const unsigned long long pre2 = s_r[2], all2 = s_r[3];
-  const long long out = st.seed ? 0 : st.cur + st.n;
-  for (int64_t i = lo + threadIdx.x; i < hi; i += kBlock) {
-    unsigned long long q = pre1 + P.loc1[i];
-    long long pos = out + (long long)(pre2 + P.loc2[i]);
+  template <class F>
+  __device__ __forceinline__ void each(const State& st, int64_t i, F f) const {
     int32_t pts[3];
-    const int np = item_points(P, st, i, pts);
-    const int32_t r = st.seed ? 0 : P.reg[P.seq[st.cur + i]];
+    const int np = points(st, i, pts);
     for (int j = 0; j < np; ++j)
-      for (unsigned long long k = P.lstart[pts[j]]; k < P.lstart[pts[j] + 1]; ++k, ++q) {
-        const int32_t d = P.links[k];
-        if (P.best[d] == q) { P.seq[pos++] = d; P.reg[d] = r; }
-      }
+      for (unsigned long long k = lstart[pts[j]]; k < lstart[pts[j] + 1]; ++k) f(links[k], j);
   }
-  team_sync<kGrid>(g);
-  st.cur = out;
-  st.n = (long long)all2;
-  st.base += (long long)all1 + 1;
-  st.depth += all2 > 0;
-  st.total += (long long)all2;
-  st.seed = 0;
-}
-
-__device__ __forceinline__ void load_state(const long long* ctl, State& st) {
-  const volatile long long* c = ctl;
-  st.n = c[0]; st.cur = c[1]; st.base = c[2]; st.depth = c[3]; st.total = c[4]; st.seed = c[5];
-}
-
-__device__ __forceinline__ void store_state(long long* ctl, const State& st) {
-  ctl[0] = st.n; ctl[1] = st.cur; ctl[2] = st.base; ctl[3] = st.depth; ctl[4] = st.total; ctl[5] = st.seed;
-}
-
-// ctl[0..5]: the starting state; ctl[6..11] and ctl[0..5] alternate as the hand-over record of each
-// single-block stretch (a block may still read one record while block 0 writes the other)
-__global__ void __launch_bounds__(kBlock) k_conn_levels(Lv P, long long* ctl) {
-  cg::grid_group g = cg::this_grid();
-  State st;
-  load_state(ctl, st);
-  int flip = 1;
-  while (st.n > 0) {
-    if (st.n <= kSmall) {
-      if (blockIdx.x == 0) {
-        do run_wave<false>(P, st, 0, 1, g); while (st.n > 0 && st.n <= kSmall);
-        if (threadIdx.x == 0) store_state(ctl + 6 * flip, st);
-      }
-      g.sync();
-      load_state(ctl + 6 * flip, st);
-      flip ^= 1;
-      continue;
-    }
-    run_wave<true>(P, st, blockIdx.x, gridDim.x, g);
+  __device__ __forceinline__ void win(const State& st, int64_t i, int, int32_t d) const {
+    reg[d] = st.seed ? 0 : reg[seq[st.cur + i]];
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) { ctl[12] = st.depth; ctl[13] = st.total; }
-}
+};
 
 // ---- ranks, PointMap, faces --------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kBlock) k_conn_sizes(const int32_t* __restrict__ seq, int64_t n,
@@ -549,19 +390,11 @@ extern "C" int b2v_conn_count(const float* verts, int64_t nv, const void* faces,
   B2V_CUDA(cudaMemcpyAsync(w.ctl, st, sizeof(st), cudaMemcpyHostToDevice, s));
 
   // every wave of every region: one persistent cooperative launch
-  int per_sm = 0;
-  B2V_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_conn_levels, kBlock, 0));
-  B2V_REQUIRE(per_sm >= 1, B2V_ERR_CUDA, "connectivity: the wave kernel does not fit on an SM");
-  if (per_sm > 2) per_sm = 2;
-  int grid = per_sm * b2v_sm_count();
-  if (grid > kMaxGrid) grid = kMaxGrid;
-  Lv P{w.tri, w.lstart, w.links, w.seeds, w.seq, w.reg, w.best, w.loc1, w.loc2, w.btot};
-  long long* ctl = w.ctl;
-  void* args[] = {&P, &ctl};
-  B2V_CUDA(cudaLaunchCooperativeKernel((const void*)k_conn_levels, dim3(grid), dim3(kBlock), args, 0, s));
-  if (int rc = b2v_check_launch("k_conn_levels")) return rc;
+  const ConnNb E{w.tri, w.lstart, w.links, w.seeds, w.seq, w.reg};
+  const WaveBufs B{w.seq, w.best, w.loc1, w.loc2, w.btot};
+  if (int rc = launch_waves(E, B, w.ctl, s, "connectivity")) return rc;
   long long res[2] = {0, 0};
-  B2V_CUDA(cudaMemcpyAsync(res, ctl + 12, sizeof(res), cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaMemcpyAsync(res, w.ctl + W_DEPTH, sizeof(res), cudaMemcpyDeviceToHost, s));
   B2V_CUDA(cudaStreamSynchronize(s));
   const long long depth = res[0], ncells = res[1];
   const long long nreg = seeded ? 1 : st[0];

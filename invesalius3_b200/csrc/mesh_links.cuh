@@ -1,13 +1,14 @@
 // The point -> cell links of a triangle mesh (vtkCellLinks), and the stable radix sort they are built with
 // (the scan is scan.cuh's). Shared by the surface tools that walk a mesh through its links (connectivity.cu,
-// smoothing.cu, fill_holes.cu); every name is in an anonymous namespace, so each translation unit has its own
-// copy.
+// smoothing.cu, fill_holes.cu, normals.cu); every name is in an anonymous namespace, so each translation unit
+// has its own copy.
 //
 //   k_conn_load   faces -> int32 [T][3] (a bad face sets ST_BAD_FACE), link counts per point.
 //   lstart        an exclusive scan of the counts: point p's links are links[lstart[p], lstart[p + 1]).
 //   links         the corners (in corner order, i.e. ascending cell) stably sorted by point id: each point's
 //                 cells in ascending id, a degenerate triangle once per corner it occupies.
 //   edge_neighbors  GetCellEdgeNeighbors through those links.
+//   uf_find / uf_unite  a lock-free union-find whose roots are the lowest ids of their sets.
 //
 // Stable sorts are LSD radix passes of 8 bits (per-block digit histograms, one scan, a scatter ranked by
 // warp match), only over the bits the largest key needs.
@@ -121,6 +122,26 @@ __device__ __forceinline__ int64_t edge_neighbors(const int32_t* __restrict__ tr
     }
   }
   return num;
+}
+
+// ---- union-find over int32 ids: a root is the lowest id of its set --------------------------------------
+__device__ __forceinline__ int32_t uf_find(const int32_t* parent, int32_t x) {
+  const volatile int32_t* p = parent;
+  int32_t y = p[x];
+  while (y != x) { x = y; y = p[x]; }
+  return x;
+}
+
+__device__ __forceinline__ void uf_unite(int32_t* parent, int32_t a, int32_t b) {
+  for (;;) {
+    a = uf_find(parent, a);
+    b = uf_find(parent, b);
+    if (a == b) return;
+    if (a > b) { const int32_t t = a; a = b; b = t; }
+    const int32_t old = atomicCAS(&parent[b], b, a);   // hook the larger root under the smaller
+    if (old == b) return;
+    b = old;
+  }
 }
 
 // Loads the faces into w.tri and builds w.lstart [V + 1] and w.links [3T] (nt > 0). W also holds status and
