@@ -616,6 +616,34 @@ int b2v_normals_emit(const float* verts, int64_t nv, int64_t nt, int face_cols, 
 int b2v_mass_properties(const float* verts, int64_t nv, const void* faces, int64_t nt, int face_cols, int faces_i64,
                         void* workspace, void* stream, double* out_host);
 
+/* ---- geodesic surface measurement -------------------------------------------------------------------------
+ * The curved measurement of the 3-D viewer (measures.py:1202-1273): vtkPointLocator::FindClosestPoint and
+ * vtkDijkstraGraphGeodesicPath on triangle cells. The contract is restated in the C checker, geodesic.c; the
+ * distances equal the sequential Dijkstra bit for bit. verts float32 or float64 (verts_f64) [nv][3]; faces int32 /
+ * int64 (faces_i64) [nt][face_cols], face_cols 3, or 4 with a leading 3. The workspace
+ * (b2v_geodesic_workspace_bytes) holds the links and one distance field.
+ *   b2v_geodesic_links      builds the point -> cell links and the bucket width; a bad face is B2V_ERR_ARG;
+ *                           synchronises. Needs nt > 0.
+ *   b2v_closest_points      picks float64 [np][3] (device) -> ids_out int64 [np] (device): the smallest
+ *                           (distance^2, id); scratch: device float64 [np]. Does not synchronise.
+ *   b2v_geodesic_distances  from start; end >= 0 stops once every point with d <= d[end] is final, end = -1
+ *                           settles the whole component (GetCumulativeWeights). dist_out float64 [nv] (device,
+ *                           may be NULL; +inf where unreached). stats_host[2] = {rounds, buckets}; synchronises.
+ *   b2v_geodesic_trace      the path of the last distances from end back to start: ids_out int64 [<= nv] and
+ *                           points_out float32 [<= nv][3] (device); counts_host[3] = {points, ambiguous steps,
+ *                           unreached (0/1)}, lengths_host[2] = {the path's length, total_in plus it, summed
+ *                           step by step}; synchronises. */
+int64_t b2v_geodesic_workspace_bytes(int64_t nv, int64_t nt);
+int b2v_geodesic_links(const void* verts, int64_t nv, int verts_f64, const void* faces, int64_t nt, int face_cols,
+                       int faces_i64, void* workspace, void* stream);
+int b2v_closest_points(const void* verts, int64_t nv, int verts_f64, const double* picks, int64_t np,
+                       double* scratch, int64_t* ids_out, void* stream);
+int b2v_geodesic_distances(const void* verts, int64_t nv, int verts_f64, int64_t nt, void* workspace, int64_t start,
+                           int64_t end, double* dist_out, void* stream, int64_t* stats_host);
+int b2v_geodesic_trace(const void* verts, int64_t nv, int verts_f64, int64_t nt, void* workspace, int64_t start,
+                       int64_t end, double total_in, int64_t* ids_out, float* points_out, void* stream,
+                       int64_t* counts_host, double* lengths_host);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

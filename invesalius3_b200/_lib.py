@@ -153,6 +153,11 @@ PROTOTYPES = {
     "b2v_normals_count": (cint, [vp, i64, vp, i64, cint, cint, dbl, cint, vp, vp, C.POINTER(i64)]),
     "b2v_normals_emit": (cint, [vp, i64, i64, cint, cint, C.POINTER(i64), vp, vp, vp, vp, vp, vp]),
     "b2v_mass_properties": (cint, [vp, i64, vp, i64, cint, cint, vp, vp, C.POINTER(dbl)]),
+    "b2v_geodesic_workspace_bytes": (i64, [i64, i64]),
+    "b2v_geodesic_links": (cint, [vp, i64, cint, vp, i64, cint, cint, vp, vp]),
+    "b2v_closest_points": (cint, [vp, i64, cint, vp, i64, vp, vp, vp]),
+    "b2v_geodesic_distances": (cint, [vp, i64, cint, i64, vp, i64, i64, vp, vp, C.POINTER(i64)]),
+    "b2v_geodesic_trace": (cint, [vp, i64, cint, i64, vp, i64, i64, dbl, vp, vp, vp, C.POINTER(i64), C.POINTER(dbl)]),
 }
 
 VIS_CAMERA_DOUBLES = 32
