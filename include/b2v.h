@@ -644,6 +644,23 @@ int b2v_geodesic_trace(const void* verts, int64_t nv, int verts_f64, int64_t nt,
                        int64_t end, double total_in, int64_t* ids_out, float* points_out, void* stream,
                        int64_t* counts_host, double* lengths_host);
 
+/* ---- volume rendering: data preparation ---------------------------------------------------------------------
+ * The arrays the 3-D volume rendering hands to VTK (Volume.LoadVolume, ApplyConvolution, volume.py:538-634).
+ * The contract (vtkImageFlip, vtkImageShiftScale, vtkImageConvolve's boundary rule, restated and unverified) is
+ * in the header of the C checker, raycasting.c; both results equal it bit for bit. Volumes dense [dz][dy][dx].
+ *   b2v_raycast_flip_shift_i16  out[z][y][x] = (uint16)(in[z][dy-1-y][x] + |min|), min = minmax_dev[0], the
+ *                               float pair b2v_minmax_f32 leaves on the device (no host round trip). in != out.
+ *                               Algorithmic bytes: 4 B per voxel.
+ *   b2v_vtk_convolve5x5_u16     one vtkImageConvolve pass with SetKernel5x5(weights_host): each slice on its own,
+ *                               float64 sums in the kernel's order, truncated to uint16. weights_host: 25 doubles
+ *                               on the HOST, passed to the kernel by value; a weight that is negative or not
+ *                               finite, or 65535 * sum >= 65536, is B2V_ERR_ARG. in != out. Algorithmic bytes:
+ *                               4 B per voxel; 25 float64 multiplies and 25 adds per voxel. */
+int b2v_raycast_flip_shift_i16(const int16_t* in, int64_t dz, int64_t dy, int64_t dx, const float* minmax_dev,
+                               uint16_t* out, void* stream);
+int b2v_vtk_convolve5x5_u16(const uint16_t* in, int64_t dz, int64_t dy, int64_t dx, const double* weights_host,
+                            uint16_t* out, void* stream);
+
 /* ---- marching cubes ---------------------------------------------------------------
  * Replaces the contour step of create_surface_piece, invesalius/data/surface_process.py:
  * 156-186 (vtkImageFlip about the origin + vtkContourFilter at iso 127 on the uint8 mask,

@@ -158,6 +158,8 @@ PROTOTYPES = {
     "b2v_closest_points": (cint, [vp, i64, cint, vp, i64, vp, vp, vp]),
     "b2v_geodesic_distances": (cint, [vp, i64, cint, i64, vp, i64, i64, vp, vp, C.POINTER(i64)]),
     "b2v_geodesic_trace": (cint, [vp, i64, cint, i64, vp, i64, i64, dbl, vp, vp, vp, C.POINTER(i64), C.POINTER(dbl)]),
+    "b2v_raycast_flip_shift_i16": (cint, [vp, i64, i64, i64, vp, vp, vp]),
+    "b2v_vtk_convolve5x5_u16": (cint, [vp, i64, i64, i64, C.POINTER(dbl), vp, vp]),
 }
 
 VIS_CAMERA_DOUBLES = 32
