@@ -9,7 +9,7 @@
 // from the valid seeds through "passable" voxels (value in [t0,t1] and out != fill) using
 // the structuring-element offsets. We compute that set in three steps:
 //   1. build   (HBM-bound, 3 B/voxel): one pass over data (+out) packs `passable` into a
-//              bit volume, 32 voxels per word along x. 512^3 voxels -> 16 MiB, i.e. the
+//              bit volume, 32 voxels per word along x (bitpack.cuh). 512^3 voxels -> 16 MiB, i.e. the
 //              whole working set of step 2 lives in the H100's 50 MB L2.
 //   2. flood   (L2 / shared-memory latency-bound): tiles of the two bit volumes are pulled
 //              into shared memory, swept once along x (run fill by the carry trick), y and
@@ -22,6 +22,7 @@
 #include <string.h>
 
 #include "b2v_common.cuh"
+#include "bitpack.cuh"
 #include "peer.cuh"
 
 namespace cg = cooperative_groups;
@@ -143,113 +144,12 @@ enum { MODE_THRESHOLD = 0, MODE_INPLACE = 1, MODE_EQUAL = 2 };
 // MODE_THRESHOLD: t0 <= data <= t1 && out != fill          (floodfill.rs:154-157)
 // MODE_INPLACE  : t0 <= data <= t1 && data != fill         (floodfill.rs:225-228)
 // MODE_EQUAL    : data == t0       && out != fill          (floodfill.rs:25)
-template <typename T, int MODE>
-__device__ __forceinline__ bool passable(T d, uint8_t o, typename Thr<T>::type t0, typename Thr<T>::type t1,
-                                         typename Thr<T>::type fill_t, uint8_t fill_o) {
-  typedef typename Thr<T>::type TT;
-  TT v = (TT)d;
-  if (MODE == MODE_EQUAL) return v == t0 && o != fill_o;
-  bool in = v >= t0 && v <= t1;
-  if (MODE == MODE_INPLACE) return in && v != fill_t;
-  return in && o != fill_o;
-}
-
-// generic build: one warp per bit word, one lane per voxel (any dtype, any alignment)
-template <typename T, int MODE>
-__global__ void __launch_bounds__(256) k_ff_build(const T* __restrict__ data, const uint8_t* __restrict__ out,
-                                                  BitVol b, typename Thr<T>::type t0, typename Thr<T>::type t1,
-                                                  typename Thr<T>::type fill_t, uint8_t fill_o,
-                                                  uint32_t* __restrict__ fg, uint32_t* __restrict__ reach) {
-  const int lane = threadIdx.x & 31;
-  const int64_t nwords = b.dz * b.dy * b.wx;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t wi = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; wi < nwords; wi += nwarps) {
-    int64_t row = wi / b.wx;
-    int w = (int)(wi - row * b.wx);
-    int64_t x = (int64_t)w * 32 + lane;
-    bool p = false;
-    if (x < b.dx) {
-      int64_t i = row * b.dx + x;
-      p = passable<T, MODE>(data[i], MODE == MODE_INPLACE ? (uint8_t)0 : out[i], t0, t1, fill_t, fill_o);
-    }
-    uint32_t bits = __ballot_sync(0xffffffffu, p);
-    if (lane == 0) {
-      fg[wi] = bits;
-      reach[wi] = 0;
-    }
-  }
-}
-
-// int16 data + uint8 out, dx % 8 == 0, 16-byte aligned rows: each lane turns one 128-bit
-// load of data (8 voxels) and one 64-bit load of out into 8 bits; 4 lanes make a word.
-// LINEAR: dx % 32 == 0, so a row holds no padding groups and group g is voxels [8g, 8g+8) and
-// byte g of the bit volume: no 64-bit division per group.
-template <int MODE, bool LINEAR>
-__global__ void __launch_bounds__(256) k_ff_build_i16_vec(const int16_t* __restrict__ data,
-                                                          const uint8_t* __restrict__ out, BitVol b, int t0, int t1,
-                                                          uint8_t fill_o, uint32_t* __restrict__ fg,
-                                                          uint32_t* __restrict__ reach) {
-  const int gx = b.wx * 4;                      // 8-voxel groups per row (padded)
-  const int64_t ngroups = b.dz * b.dy * gx;     // multiple of 4
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
-  const int lane = threadIdx.x & 31;
-  // passable = lo <= v <= hi (MODE_EQUAL: lo = hi = t0) and out != fill, eight voxels at a time
-  const int lo = MODE == MODE_EQUAL ? t0 : (t0 < -32768 ? -32768 : t0);
-  const int hi = MODE == MODE_EQUAL ? t0 : (t1 > 32767 ? 32767 : t1);
-  const bool none = lo > hi || lo > 32767 || hi < -32768;
-  const uint32_t lo2 = ((uint32_t)lo & 0xffffu) * 0x00010001u, hi2 = ((uint32_t)hi & 0xffffu) * 0x00010001u;
-  const uint32_t fill4 = (uint32_t)fill_o * 0x01010101u;
-  // four groups per thread and iteration: 4 x (128-bit + 64-bit) loads in flight
-  for (int64_t g0 = (int64_t)blockIdx.x * blockDim.x * 4; g0 < ngroups; g0 += stride) {
-    int4 v[4];
-    uint2 o[4];
-    int64_t row[4];
-    int q[4];
-    bool ok[4], in[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int64_t g = g0 + k * blockDim.x + threadIdx.x;
-      ok[k] = g < ngroups;
-      if (LINEAR) {
-        row[k] = 0;
-        q[k] = 0;
-        in[k] = ok[k];
-      } else {
-        row[k] = ok[k] ? g / gx : 0;
-        q[k] = ok[k] ? (int)(g - row[k] * gx) : 0;
-        in[k] = ok[k] && (int64_t)q[k] * 8 < b.dx;
-      }
-      v[k] = make_int4(0, 0, 0, 0);
-      o[k] = make_uint2(0u, 0u);
-      if (in[k]) {
-        const int64_t i = LINEAR ? g * 8 : row[k] * b.dx + (int64_t)q[k] * 8;
-        v[k] = ld_stream((const int4*)(data + i));
-        o[k] = ld_stream((const uint2*)(out + i));
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      uint32_t bits = 0;
-      if (in[k] && !none) {
-        // voxels 0..3 / 4..7 as 0x80-per-byte flags: in range AND out != fill
-        const uint32_t a = __byte_perm(inrange_flags_s16x2((uint32_t)v[k].x, lo2, hi2),
-                                       inrange_flags_s16x2((uint32_t)v[k].y, lo2, hi2), 0x7531);
-        const uint32_t c = __byte_perm(inrange_flags_s16x2((uint32_t)v[k].z, lo2, hi2),
-                                       inrange_flags_s16x2((uint32_t)v[k].w, lo2, hi2), 0x7531);
-        bits = flags_to_nibble(a & nonzero_flags_u8x4(o[k].x ^ fill4)) |
-               (flags_to_nibble(c & nonzero_flags_u8x4(o[k].y ^ fill4)) << 4);
-      }
-      uint32_t word = bits << (8 * (lane & 3));
-      word |= __shfl_xor_sync(0xffffffffu, word, 1);
-      word |= __shfl_xor_sync(0xffffffffu, word, 2);
-      if ((lane & 3) == 0 && ok[k]) {
-        const int64_t wi = LINEAR ? (g0 + k * blockDim.x + threadIdx.x) >> 2 : row[k] * b.wx + (q[k] >> 2);
-        fg[wi] = word;
-        reach[wi] = 0;
-      }
-    }
-  }
-}
+// The first and the last are InRange (bitpack.cuh) with `out` as its other stream; the in-place test is this one.
+template <typename B>
+struct InRangeNotFill {
+  B lo, hi, fill;
+  __device__ __forceinline__ bool operator()(B v, int64_t) const { return v >= lo && v <= hi && v != fill; }
+};
 
 // seeds: (x, y, z) triples, already bounds-checked on the host. A valid seed is reached
 // and passable even if out already holds `fill` there (floodfill.rs:121-127); force=1
@@ -1221,21 +1121,13 @@ int flood(T* data, uint8_t* out, int64_t dz, int64_t dy, int64_t dx, const int64
     // control region (active flags, round flags) starts clean
     B2V_CUDA(cudaMemsetAsync(w.active[0], 0, (size_t)((char*)w.seeds - (char*)w.active[0]), s));
     if (nseeds) B2V_CUDA(cudaMemcpyAsync(w.seeds, seeds_host, (size_t)nseeds * 24, cudaMemcpyHostToDevice, s));
-    bool vec = sizeof(T) == 2 && MODE != MODE_INPLACE && dx % 8 == 0 && b2v_aligned16(data) &&
-               ((uintptr_t)out & 7u) == 0;
-    if (vec) {
-      if (dx % 32 == 0)
-        k_ff_build_i16_vec<MODE, true><<<b2v_grid(nwords * 4, 1024, 16), 256, 0, s>>>((const int16_t*)data, out, b,
-                                                                                      (int)t0, (int)t1, fill_o, w.fg,
-                                                                                      w.reach);
-      else
-        k_ff_build_i16_vec<MODE, false><<<b2v_grid(nwords * 4, 1024, 16), 256, 0, s>>>((const int16_t*)data, out, b,
-                                                                                       (int)t0, (int)t1, fill_o, w.fg,
-                                                                                       w.reach);
-    } else {
-      k_ff_build<T, MODE><<<b2v_grid(nwords, 8, 16), 256, 0, s>>>(data, out, b, t0, t1, fill_t, fill_o, w.fg, w.reach);
-    }
-    if ((rc = b2v_check_launch("k_ff_build"))) return rc;
+    typedef typename Thr<T>::type TT;
+    if (MODE == MODE_INPLACE)
+      rc = pack_bits<T>(data, dz * dy, dx, InRangeNotFill<TT>{t0, t1, fill_t}, w.fg, w.reach, s);
+    else
+      rc = pack_bits<T>(data, dz * dy, dx, InRange<TT, true>{t0, MODE == MODE_EQUAL ? t0 : t1, out, fill_o}, w.fg,
+                        w.reach, s);
+    if (rc) return rc;
     if (nseeds) {
       k_ff_seeds<T><<<(unsigned)ceil_div64(nseeds, 128), 128, 0, s>>>(data, b, w.seeds, nseeds, t0, t1,
                                                                       MODE == MODE_EQUAL ? 1 : 0, w.fg, w.reach,

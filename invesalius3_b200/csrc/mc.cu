@@ -4,7 +4,7 @@
 // restated by the CPU checker; VTK itself is not available, so parity to VTK is unpinned.
 //
 //   1. bits   (HBM-bound, the only pass over the volume: 1 B/voxel uint8, 2 B/voxel int16):
-//             inside(p) = S[p] >= iso packed 32 voxels per word along x.
+//             inside(p) = S[p] >= iso packed 32 voxels per word along x (bitpack.cuh).
 //   2. classify + compact (on bits, L2 resident, ONE pass): per word the crossing masks towards
 //             +x/+y/+z, the owned vertices (popcounts) and the triangles of its active cells;
 //             non-empty words are appended in word order to two compact lists, the running
@@ -13,6 +13,7 @@
 //             vertex id is  voff[owner word] + popcounts below the owner bit, each owner
 //             record fetched once per cell.
 #include "b2v_common.cuh"
+#include "bitpack.cuh"
 #include "peer.cuh"
 #define B2V_MC_QUAL __device__
 #include "mc_tables.h"
@@ -82,105 +83,6 @@ McWs carve(void* base, const McGeom& g) {
   w.ctl_bytes = off - ctl0;
   w.bytes = off;
   return w;
-}
-
-// ---- 1. inside bits ---------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) k_mc_bits(const T* __restrict__ vol, McGeom g, int ithr,
-                                                 uint32_t* __restrict__ bits) {
-  const int lane = threadIdx.x & 31;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t wi = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; wi < g.nwords; wi += nwarps) {
-    int64_t row = wi / g.wx;
-    int64_t x = (wi - row * g.wx) * 32 + lane;
-    bool in = x < g.nx && (int)vol[row * g.nx + x] >= ithr;
-    uint32_t b = __ballot_sync(0xffffffffu, in);
-    if (lane == 0) bits[wi] = b;
-  }
-}
-
-// uint8, nx % 16 == 0, aligned: one 128-bit load = 16 voxels per lane, 2 lanes per word.
-// LINEAR: nx % 32 == 0, rows hold no padding groups: group gi is voxels [16 gi, 16 gi + 16)
-// and half-word gi of the bit volume (no 64-bit division per group).
-template <bool LINEAR>
-__global__ void __launch_bounds__(256) k_mc_bits_u8_vec(const uint8_t* __restrict__ vol, McGeom g, int ithr,
-                                                        uint32_t* __restrict__ bits) {
-  const int gx = g.wx * 2;  // 16-voxel groups per row (padded)
-  const int64_t ngroups = g.nz * g.ny * gx;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
-  const int lane = threadIdx.x & 31;
-  const uint32_t thr = (uint32_t)(ithr > 255 ? 255 : (ithr < 0 ? 0 : ithr));
-  const uint32_t t7 = (thr & 0x7fu) * 0x01010101u;
-  const bool t_high = thr >= 128u;
-  const bool none = ithr > 255;
-  // four 128-bit loads in flight per thread; bytes are compared four at a time
-  for (int64_t g0 = (int64_t)blockIdx.x * blockDim.x * 4; g0 < ngroups; g0 += stride) {
-    uint4 v[4];
-    int64_t row[4];
-    int q[4];
-    bool ok[4], in[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int64_t gi = g0 + k * blockDim.x + threadIdx.x;
-      ok[k] = gi < ngroups;
-      if (LINEAR) {
-        row[k] = 0; q[k] = 0;
-        in[k] = ok[k];
-      } else {
-        row[k] = ok[k] ? gi / gx : 0;
-        q[k] = ok[k] ? (int)(gi - row[k] * gx) : 0;
-        in[k] = ok[k] && (int64_t)q[k] * 16 < g.nx;   // a padded group contributes zero bits
-      }
-      v[k] = make_uint4(0u, 0u, 0u, 0u);
-      if (in[k]) v[k] = ld_stream((const uint4*)(vol + (LINEAR ? gi * 16 : row[k] * g.nx + (int64_t)q[k] * 16)));
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      uint32_t b = 0;
-      if (in[k] && !none) {
-        b = flags_to_nibble(ge_flags_u8x4(v[k].x, t7, t_high)) | (flags_to_nibble(ge_flags_u8x4(v[k].y, t7, t_high)) << 4) |
-            (flags_to_nibble(ge_flags_u8x4(v[k].z, t7, t_high)) << 8) |
-            (flags_to_nibble(ge_flags_u8x4(v[k].w, t7, t_high)) << 12);
-      }
-      uint32_t word = b << (16 * (lane & 1));
-      word |= __shfl_xor_sync(0xffffffffu, word, 1);
-      if ((lane & 1) == 0 && ok[k]) {
-        const int64_t gi = g0 + k * blockDim.x + threadIdx.x;
-        bits[LINEAR ? gi >> 1 : row[k] * g.wx + (q[k] >> 1)] = word;
-      }
-    }
-  }
-}
-
-// int16, nx % 8 == 0, aligned: 8 voxels per lane, 4 lanes per word
-__global__ void __launch_bounds__(256) k_mc_bits_i16_vec(const int16_t* __restrict__ vol, McGeom g, int ithr,
-                                                         uint32_t* __restrict__ bits) {
-  const int gx = g.wx * 4;
-  const int64_t ngroups = g.nz * g.ny * gx;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int lane = threadIdx.x & 31;
-  for (int64_t g0 = (int64_t)blockIdx.x * blockDim.x; g0 < ngroups; g0 += stride) {
-    int64_t gi = g0 + threadIdx.x;
-    uint32_t b = 0;
-    int64_t row = 0;
-    int q = 0;
-    if (gi < ngroups) {
-      row = gi / gx;
-      q = (int)(gi - row * gx);
-      int64_t x = (int64_t)q * 8;
-      if (x < g.nx) {
-        int4 v = ld_stream((const int4*)(vol + row * g.nx + x));
-        int vv[8] = {(int16_t)(v.x & 0xffff), v.x >> 16, (int16_t)(v.y & 0xffff), v.y >> 16,
-                     (int16_t)(v.z & 0xffff), v.z >> 16, (int16_t)(v.w & 0xffff), v.w >> 16};
-#pragma unroll
-        for (int k = 0; k < 8; ++k) b |= (uint32_t)(vv[k] >= ithr) << k;
-      }
-    }
-    uint32_t word = b << (8 * (lane & 3));
-    word |= __shfl_xor_sync(0xffffffffu, word, 1);
-    word |= __shfl_xor_sync(0xffffffffu, word, 2);
-    if ((lane & 3) == 0 && gi < ngroups) bits[row * g.wx + (q >> 2)] = word;
-  }
 }
 
 // ---- 2. classify (one pass over the bits, per-TILE counts, scan of the tile counts) ----------
@@ -757,23 +659,14 @@ static int mc_count_impl(const void* vol, int dtype, int64_t nz, int64_t ny, int
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
   B2V_CUDA(cudaMemsetAsync(w.totals, 0, (size_t)w.ctl_bytes, s));
-  if (dtype == B2V_U8) {
-    int thr = int_threshold(iso, 0, 255);
-    if (nx % 16 == 0 && b2v_aligned16(vol))
-      if (nx % 32 == 0)
-        k_mc_bits_u8_vec<true><<<b2v_grid(g.nwords * 2, 1024, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
-      else
-        k_mc_bits_u8_vec<false><<<b2v_grid(g.nwords * 2, 1024, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
-    else
-      k_mc_bits<uint8_t><<<b2v_grid(g.nwords, 8, 16), 256, 0, s>>>((const uint8_t*)vol, g, thr, w.bits);
-  } else {
-    int thr = int_threshold(iso, -32768, 32767);
-    if (nx % 8 == 0 && b2v_aligned16(vol))
-      k_mc_bits_i16_vec<<<b2v_grid(g.nwords * 4, 256, 16), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
-    else
-      k_mc_bits<int16_t><<<b2v_grid(g.nwords, 8, 16), 256, 0, s>>>((const int16_t*)vol, g, thr, w.bits);
-  }
-  if ((rc = b2v_check_launch("k_mc_bits"))) return rc;
+  // inside <=> S >= int_threshold(iso) <=> S in [int_threshold(iso), dtype max]
+  if (dtype == B2V_U8)
+    rc = pack_bits((const uint8_t*)vol, nz * ny, nx, InRange<int, false>{int_threshold(iso, 0, 255), 255, nullptr, 0},
+                   w.bits, nullptr, s);
+  else
+    rc = pack_bits((const int16_t*)vol, nz * ny, nx,
+                   InRange<int, false>{int_threshold(iso, -32768, 32767), 32767, nullptr, 0}, w.bits, nullptr, s);
+  if (rc) return rc;
   const int ntiles = (int)ceil_div64(g.nwords, kTileWords);
   if (g.wx % 4 == 0)
     k_mc_classify<true><<<ntiles, kTileThreads, 0, s>>>(w.bits, g, skip_last, w.vrec, w.tcnt, w.toff, w.ticket,

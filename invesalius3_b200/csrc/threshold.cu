@@ -9,11 +9,9 @@
 
 namespace {
 
-// 0xFF in every byte of `x` that is zero, 0x00 elsewhere (exact, no cross-byte borrow).
+// 0xFF in every byte of `x` that is zero, 0x00 elsewhere
 __device__ __forceinline__ uint32_t zero_bytes_ff(uint32_t x) {
-  uint32_t t = (x & 0x7f7f7f7fu) + 0x7f7f7f7fu;
-  t = ~(t | x | 0x7f7f7f7fu);  // 0x80 where the byte was zero
-  return (t >> 7) * 0xffu;
+  return ((nonzero_flags_u8x4(x) ^ 0x80808080u) >> 7) * 0xffu;
 }
 
 // bytes of `m` equal to 1, 2, 253 or 254 -> 0xFF
@@ -26,11 +24,7 @@ __device__ __forceinline__ uint32_t marker_bytes_ff(uint32_t m) {
 
 // two packed int16 voxels -> 0xFFFF per half that lies in [lo, hi]
 __device__ __forceinline__ uint32_t inrange_s16x2(uint32_t w, uint32_t lo2, uint32_t hi2) {
-  uint32_t c = max_s16x2(min_s16x2(w, hi2), lo2);
-  uint32_t d = c ^ w;  // half == 0  <=>  in range
-  uint32_t t = (d & 0x7fff7fffu) + 0x7fff7fffu;
-  t = ~(t | d | 0x7fff7fffu);  // 0x8000 where the half was zero
-  return (t >> 15) * 0xffffu;
+  return (inrange_flags_s16x2(w, lo2, hi2) >> 15) * 0xffffu;
 }
 
 __device__ __forceinline__ uint32_t thr4(uint32_t w0, uint32_t w1, uint32_t lo2, uint32_t hi2) {

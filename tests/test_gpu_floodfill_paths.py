@@ -1,6 +1,6 @@
 """Flood-fill paths that the parity tests of test_gpu_floodfill.py do not reach: every tuning knob
 (each in a process of its own), more than 1024 tiles, floods of thousands of rounds and the round
-cap, and int16 data and thresholds at their limits through every build of the bit volumes.
+cap, and int16 and uint8 data and thresholds at their limits through every build of the bit volumes.
 
 Every device result is compared bit for bit with the serial C checker; where the element is
 symmetric and the volume large, also with the seeded components of the passable set that
@@ -17,6 +17,7 @@ import pytest
 from scipy import ndimage
 from scipy.ndimage import generate_binary_structure
 
+import bitpack_model
 import ff_knob_child as knob
 
 pytestmark = pytest.mark.gpu
@@ -239,7 +240,7 @@ FILL = 1
 THRESHOLDS = [(-32768, -32768), (32767, 32767), (-32768, 32767), (-32767, 32766), (0, 0), (5, 4),
               (-40000, -32768), (32767, 40000), (-0.5, 0.5)]
 # name -> (dx, data offset in elements, out offset in bytes). 512: the vectorised build with
-# dx % 32 == 0; 200: vectorised, padded rows; the rest take the generic build.
+# dx % 32 == 0; 200: vectorised, padded rows; the rest take the ballot build (bitpack_model).
 LAYOUTS = {"dx512": (512, 0, 0), "dx200": (200, 0, 0), "dx203": (203, 0, 0), "data+1": (512, 1, 0),
            **{f"out+{k}": (512, 0, k) for k in range(1, 8)}}
 LIMIT_ELEMENTS = [generate_binary_structure(3, 1), generate_binary_structure(3, 3), generate_binary_structure(3, 2)]
@@ -417,3 +418,106 @@ def test_threshold_int16_limits(orc, layout):
             dev.threshold(d, lo, hi, o, keep)
             got = o.cpu().numpy()
             assert np.array_equal(got, want), (layout, lo, hi, keep, int((got != want).sum()))
+
+
+# ----------------------------------------------------------------- E. uint8 limits, build matrix
+U8_THRESHOLDS = [(0, 0), (255, 255), (0, 255), (127, 128), (128, 255), (0, 127), (1, 254), (128, 127), (-40, 0),
+                 (255, 400), (-40, -1), (256, 400), (-0.5, 0.5), (127.2, 127.8)]
+# as LAYOUTS for uint8 data: 512 and 208 (a multiple of 16 with padded rows) take the vectorised build, the widths
+# 200 and 203, the misaligned data and every misaligned out (16-byte loads) the ballot build
+U8_LAYOUTS = {"dx512": (512, 0, 0), "dx208": (208, 0, 0), "dx200": (200, 0, 0), "dx203": (203, 0, 0),
+              "data+1": (512, 1, 0), **{f"out+{k}": (512, 0, k) for k in range(1, 16)}}
+# equality flood values: both limits, the two plateaus, a non-integer and two outside uint8 (these three match
+# nothing; the seed is still marked)
+U8_EQUAL_VALUES = [0, 255, 127, 128, 0.5, 300, -1]
+
+
+def test_layouts_reach_every_packing_kernel():
+    """The flood's build matrices reach every packing kernel, and each vectorised one again with a
+    misaligned data or out pointer (the ballot at that width)."""
+    cases = [(np.int16, dx, 2 * doff, ooff) for dx, doff, ooff in LAYOUTS.values()]
+    cases += [(np.uint8, dx, doff, ooff) for dx, doff, ooff in U8_LAYOUTS.values()]
+    assert {bitpack_model.pack_kernel(*c) for c in cases} == set(bitpack_model.VEC + bitpack_model.BALLOT)
+    misaligned = {bitpack_model.pack_kernel(dt, dx) for dt, dx, doff, ooff in cases
+                  if bitpack_model.pack_kernel(dt, dx, doff, ooff).startswith("ballot<")}
+    assert misaligned >= {"vec<int16,linear>", "vec<uint8,linear>"}
+    assert {ooff for dt, dx, doff, ooff in cases if dt == np.uint8} >= set(range(16))
+
+
+def _limits_volume_u8(dx):
+    """(15, 63, dx) uint8: smooth noise saturated at 0 and 255 over a fifth of the volume, plateaus at 127
+    and 128, and the first 512 voxels (raveled) holding every value twice in order; out as in
+    _limits_volume."""
+    def make():
+        shape = (15, 63, dx)
+        rng = np.random.default_rng(1000 + dx)
+        f = ndimage.gaussian_filter(rng.normal(size=shape), 3.0)
+        f /= np.quantile(np.abs(f), 0.8)
+        v = np.clip(np.rint(127.5 + f * 127.5), 0, 255)
+        v[np.abs(v - 127.5) < 30] = np.where(v[np.abs(v - 127.5) < 30] < 127.5, 127, 128)
+        v = v.astype(np.uint8)
+        v.reshape(-1)[:512] = np.tile(np.arange(256), 2)
+        out0 = np.zeros(shape, np.uint8)
+        for val, p in ((FILL, 0.02), (2, 0.01), (200, 0.01), (253, 0.01), (254, 0.01)):
+            out0[rng.random(shape) < p] = val
+        return v, out0
+    return _memo(("limits-u8", dx), make)
+
+
+@pytest.mark.parametrize("layout", list(U8_LAYOUTS))
+def test_floodfill_threshold_uint8_limits(orc, engine, layout):
+    from invesalius3_b200 import device as dev
+    dx, doff, ooff = U8_LAYOUTS[layout]
+    data, out0 = _limits_volume_u8(dx)
+    d = _placed(data, doff)
+    for i, (t0, t1) in enumerate(U8_THRESHOLDS):
+        st = LIMIT_ELEMENTS[i % 3]
+        seeds = _seeds_in(data, t0, t1, np.random.default_rng(i))
+
+        def reference():   # the checker on float64 data: any bound, exactly
+            want = out0.copy()
+            orc._floodfill_threshold_core(data.astype(np.float64), seeds, float(t0), float(t1), FILL,
+                                          np.ascontiguousarray(st, np.uint8), want)
+            return want
+        want = _memo(("thr-u8", dx, i), reference)
+        if _nonempty(data, t0, t1):
+            assert ((want == FILL) & (out0 != FILL)).sum() > 1000, (t0, t1)
+        else:
+            assert np.array_equal(want, out0)
+        o = _placed(out0, ooff)
+        dev.floodfill_threshold(d, seeds, t0, t1, FILL, st, o)
+        got = o.cpu().numpy()
+        assert np.array_equal(got, want), (layout, t0, t1, int((got != want).sum()))
+
+
+@pytest.mark.parametrize("layout", list(U8_LAYOUTS))
+def test_floodfill_equal_uint8_limits(orc, engine, layout):
+    from invesalius3_b200 import device as dev
+    dx, doff, ooff = U8_LAYOUTS[layout]
+    data, out0 = _limits_volume_u8(dx)
+    d = _placed(data, doff)
+    for v in U8_EQUAL_VALUES:
+        # seed in the largest 6-connected region of data == v (any voxel if there is none)
+        lab, n = ndimage.label((data == v) & (out0 != FILL))
+        if n:
+            idx = np.flatnonzero(lab == 1 + np.argmax(np.bincount(lab.ravel())[1:]))
+            i = idx[idx.size // 2]
+        else:
+            idx, i = np.array([]), data.size // 3
+        z, y, x = (int(c) for c in np.unravel_index(i, data.shape))
+
+        def reference():
+            want = out0.copy()
+            orc.floodfill(data.astype(np.float64), x, y, z, float(v), FILL, want)
+            return want
+        want = _memo(("eq-u8", dx, v), reference)
+        if idx.size:
+            assert ((want == FILL) & (out0 != FILL)).sum() > 500, v
+        else:
+            expect = out0.copy()
+            expect[z, y, x] = FILL
+            assert np.array_equal(want, expect)
+        o = _placed(out0, ooff)
+        dev.floodfill(d, x, y, z, v, FILL, o)
+        got = o.cpu().numpy()
+        assert np.array_equal(got, want), (layout, v, int((got != want).sum()))
