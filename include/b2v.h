@@ -505,6 +505,44 @@ int b2v_visibility_emit(const float* verts, int64_t nv, const void* faces, int64
                         int nviews, int remove_visible, void* workspace, float* verts_out, int32_t* faces_out,
                         void* stream);
 
+/* ---- clean and triangulate surfaces ---------------------------------------------------------------
+ * vtkCleanPolyData at InVesalius's settings (tolerance 0, unused points removed, polys -> lines -> verts,
+ * strips -> polys -> lines -> verts) and vtkTriangleFilter, on the polys and strips of a surface. The rules
+ * (restated from VTK 9.3, unverified) are in the header of the C checker, clean.c.
+ *   Each cell family (polys, strips) is conn, offs, n cells, nconn corners, form, i64: form 0 is VTK 9's
+ *   offsets int64 [n + 1] + connectivity [nconn]; form 3 is faces [n][3] and form 4 faces [n][4] with a
+ *   leading 3 (offs NULL, nconn = 3 n). Ids are int32 (i64 = 0) or int64. verts: float32 [nv][3], nv < 2^31.
+ *   Malformed offsets and ids outside [0, nv) are B2V_ERR_ARG.
+ *   b2v_clean_count    counts_host[7] = {points, verts, lines, polys, poly corners, strips, strip corners}.
+ *                      Synchronises the stream.
+ *   b2v_clean_emit     from the same workspace: points_out float32 [points][3] in order of first use,
+ *                      point_ids_out int64 (their input points); vconn_out, lconn_out int64 (one and two
+ *                      points a cell); poffs_out / soffs_out int64 [cells + 1] and pconn_out / sconn_out;
+ *                      cell_ids_out int64: the input cell (polys numbered first, then strips) of every
+ *                      output cell, in the order verts, lines, polys, strips.
+ *   b2v_triangle_filter_count  counts_host[1] = {triangles}; polys of more than 3 points are clipped by
+ *                      vtkPolygon's ear cut (a polygon it cannot finish gives fewer than n - 2). The workspace
+ *                      query takes the cells and the polys' corners. Synchronises the stream.
+ *   b2v_triangle_filter_emit   tris_out int64 [triangles][3]: the polys' triangles, then each strip's n - 2
+ *                      in vtkTriangleStrip's alternating winding; cell_ids_out int64 [triangles]. */
+int64_t b2v_clean_workspace_bytes(int64_t nv, int64_t ncells, int64_t ncorners);
+int b2v_clean_count(const float* verts, int64_t nv, const void* pconn, const int64_t* poffs, int64_t np, int64_t npconn,
+                    int pform, int pi64, const void* sconn, const int64_t* soffs, int64_t ns, int64_t nsconn, int sform,
+                    int si64, void* workspace, void* stream, int64_t* counts_host);
+int b2v_clean_emit(const float* verts, int64_t nv, const void* pconn, const int64_t* poffs, int64_t np, int64_t npconn,
+                   int pform, int pi64, const void* sconn, const int64_t* soffs, int64_t ns, int64_t nsconn, int sform,
+                   int si64, void* workspace, float* points_out, int64_t* point_ids_out, int64_t* vconn_out,
+                   int64_t* lconn_out, int64_t* poffs_out, int64_t* pconn_out, int64_t* soffs_out, int64_t* sconn_out,
+                   int64_t* cell_ids_out, void* stream);
+int64_t b2v_triangle_filter_workspace_bytes(int64_t ncells, int64_t npoly_corners);
+int b2v_triangle_filter_count(const float* verts, int64_t nv, const void* pconn, const int64_t* poffs, int64_t np,
+                              int64_t npconn, int pform, int pi64, const void* sconn, const int64_t* soffs, int64_t ns,
+                              int64_t nsconn, int sform, int si64, void* workspace, void* stream, int64_t* counts_host);
+int b2v_triangle_filter_emit(const float* verts, int64_t nv, const void* pconn, const int64_t* poffs, int64_t np,
+                             int64_t npconn, int pform, int pi64, const void* sconn, const int64_t* soffs, int64_t ns,
+                             int64_t nsconn, int sform, int si64, void* workspace, int64_t* tris_out,
+                             int64_t* cell_ids_out, void* stream);
+
 /* ---- surface connectivity ------------------------------------------------------------------------
  * vtkPolyDataConnectivityFilter on triangles, behind polydata_utils.SelectLargestPart, SplitDisconectedParts
  * and JoinSeedsParts (invesalius/data/polydata_utils.py:206-278; surface.py:319-411). The contract (VTK's

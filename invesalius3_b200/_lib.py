@@ -135,6 +135,16 @@ PROTOTYPES = {
     "b2v_visibility_count": (cint, [vp, i64, vp, i64, cint, cint, C.POINTER(dbl), cint, cint, vp, vp, C.POINTER(i64),
                                     C.POINTER(i64)]),
     "b2v_visibility_emit": (cint, [vp, i64, vp, i64, cint, cint, cint, cint, vp, vp, vp, vp]),
+    "b2v_clean_workspace_bytes": (i64, [i64, i64, i64]),
+    "b2v_clean_count": (cint, [vp, i64, vp, vp, i64, i64, cint, cint, vp, vp, i64, i64, cint, cint, vp, vp,
+                               C.POINTER(i64)]),
+    "b2v_clean_emit": (cint, [vp, i64, vp, vp, i64, i64, cint, cint, vp, vp, i64, i64, cint, cint, vp, vp, vp, vp, vp,
+                              vp, vp, vp, vp, vp, vp]),
+    "b2v_triangle_filter_workspace_bytes": (i64, [i64, i64]),
+    "b2v_triangle_filter_count": (cint, [vp, i64, vp, vp, i64, i64, cint, cint, vp, vp, i64, i64, cint, cint, vp, vp,
+                                         C.POINTER(i64)]),
+    "b2v_triangle_filter_emit": (cint, [vp, i64, vp, vp, i64, i64, cint, cint, vp, vp, i64, i64, cint, cint, vp, vp,
+                                        vp, vp]),
     "b2v_conn_workspace_bytes": (i64, [i64, i64, i64]),
     "b2v_conn_layout": (cint, [i64, i64, i64, C.POINTER(i64)]),
     "b2v_conn_count": (cint, [vp, i64, vp, i64, cint, cint, cint, vp, i64, vp, vp, C.POINTER(i64)]),

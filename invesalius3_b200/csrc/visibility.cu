@@ -15,9 +15,9 @@
 //                      queued for k_vis_raster_big, so a coarse mesh never serialises a warp.
 //   k_vis_raster_big   a persistent grid; one block per queued triangle, its threads stride the box.
 //   k_vis_points       one thread per vertex: z_w < zbuf + tolerance in any view.
-//   k_vis_merge_insert exactly coincident vertices share one slot of an open-addressing hash table
-//                      (keys: the coordinate bits with -0 read as +0, compared with float ==).
-//   k_vis_first_use    atomicMin of the corner index over the kept faces, per slot.
+//   k_merge_insert     exactly coincident vertices share one slot of an open-addressing hash table
+//                      (mesh_merge.cuh, shared with the clean of clean.cu).
+//   k_vis_first_use    note_first_use: atomicMin of the corner index over the kept faces, per slot.
 //   k_vis_block_counts / k_scan_sums / k_vis_emit_*   the O(T) compaction: a corner is the first
 //                      use of its (merged) vertex when its index is that minimum; scans of those flags
 //                      number the output vertices, scans of the kept, non-degenerate faces order them.
@@ -28,6 +28,7 @@
 #include <string.h>
 
 #include "b2v_common.cuh"
+#include "mesh_merge.cuh"
 #include "scan.cuh"
 
 namespace {
@@ -191,18 +192,12 @@ struct VisWs {
   size_t bytes;
 };
 
-uint64_t hash_slots(int64_t nv) {
-  uint64_t h = 1024;
-  while (h < 2 * (uint64_t)nv) h <<= 1;
-  return h;
-}
-
 VisWs carve(void* base, int64_t nv, int64_t nt, int nviews) {
   VisWs w;
   char* p = (char*)base;
   size_t o = 0;
   auto take = [&](size_t n) { char* r = p + o; o += align256(n); return r; };
-  const uint64_t H = hash_slots(nv);
+  const uint64_t H = merge_slots(nv);
   w.hmask = H - 1;
   w.nb = ceil_div64(nt, kBlock);
   w.misc = (uint32_t*)take(64);
@@ -223,7 +218,6 @@ VisWs carve(void* base, int64_t nv, int64_t nt, int nviews) {
 }
 
 // ---- device helpers ---------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t canon_bits(float f) { return __float_as_uint(f == 0.0f ? 0.0f : f); }
 __device__ __forceinline__ uint32_t order_key(float f) {
   const uint32_t u = canon_bits(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
@@ -402,30 +396,6 @@ __global__ void __launch_bounds__(kBlock) k_vis_points(int64_t nv, int nviews, c
   }
 }
 
-// ---- point merge ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t vhash(uint32_t a, uint32_t b, uint32_t c) {
-  uint64_t h = (uint64_t)a * 0x9E3779B97F4A7C15ull ^ (uint64_t)b * 0xC2B2AE3D27D4EB4Full ^ (uint64_t)c * 0x165667B19E3779F9ull;
-  h ^= h >> 31;
-  h *= 0xBF58476D1CE4E5B9ull;
-  h ^= h >> 29;
-  return h;
-}
-
-__global__ void __launch_bounds__(kBlock) k_vis_merge_insert(const float* __restrict__ v, int64_t nv, uint64_t hmask,
-                                                             int32_t* slots, uint32_t* __restrict__ rep) {
-  for (int64_t k = gtid(); k < nv; k += gstride()) {
-    const float x = v[3 * k], y = v[3 * k + 1], z = v[3 * k + 2];
-    uint64_t h = vhash(canon_bits(x), canon_bits(y), canon_bits(z)) & hmask;
-    for (;;) {
-      const int32_t old = atomicCAS(&slots[h], -1, (int32_t)k);
-      if (old == -1) break;
-      if (v[3 * (int64_t)old] == x && v[3 * (int64_t)old + 1] == y && v[3 * (int64_t)old + 2] == z) break;
-      h = (h + 1) & hmask;
-    }
-    rep[k] = (uint32_t)h;
-  }
-}
-
 // ---- face selection and compaction ------------------------------------------------------------------------
 __device__ __forceinline__ bool face_kept(const Faces& F, int64_t t, const uint8_t* __restrict__ vis, uint8_t flip,
                                           int64_t v[3]) {
@@ -439,11 +409,7 @@ __global__ void __launch_bounds__(kBlock) k_vis_first_use(Faces F, const uint8_t
   for (int64_t t = gtid(); t < F.nt; t += gstride()) {
     int64_t v[3];
     if (!face_kept(F, t, vis, flip, v)) continue;
-    for (int c = 0; c < 3; ++c) {
-      unsigned long long* f = first + rep[v[c]];
-      const unsigned long long corner = (unsigned long long)(3 * t + c);
-      if (corner < *f) atomicMin(f, corner);
-    }
+    for (int c = 0; c < 3; ++c) note_first_use(first, rep[v[c]], (unsigned long long)(3 * t + c));
   }
 }
 
@@ -463,7 +429,7 @@ __device__ __forceinline__ FaceFlags face_flags(const Faces& F, int64_t t, const
   if (t >= F.nt || !face_kept(F, t, vis, flip, o.v)) return o;
   for (int c = 0; c < 3; ++c) {
     o.r[c] = rep[o.v[c]];
-    if (first[o.r[c]] == (unsigned long long)(3 * t + c)) o.corners |= 1u << c;
+    if (is_first_use(first, o.r[c], (unsigned long long)(3 * t + c))) o.corners |= 1u << c;
   }
   o.emit = o.r[0] != o.r[1] && o.r[1] != o.r[2] && o.r[0] != o.r[2];
   return o;
@@ -623,16 +589,14 @@ extern "C" int b2v_visibility_count(const float* verts, int64_t nv, const void* 
   B2V_CUDA(cudaMemsetAsync(w.misc, 0, 64, s));
   B2V_CUDA(cudaMemsetAsync(w.totals, 0, 16, s));
   B2V_CUDA(cudaMemsetAsync(w.qcount, 0, 8, s));
-  B2V_CUDA(cudaMemsetAsync(w.slots, 0xff, (w.hmask + 1) * 4, s));
-  B2V_CUDA(cudaMemsetAsync(w.first, 0xff, (w.hmask + 1) * 8, s));
+  if (int rc = merge_reset(w.slots, w.first, w.hmask + 1, s)) return rc;
 
   k_fill<unsigned long long><<<b2v_grid((int64_t)nviews * kPix, kBlock, 8), kBlock, 0, s>>>(
       w.zbuf, (int64_t)nviews * kPix, kDepthOne);
   if (int rc = b2v_check_launch("k_fill")) return rc;
   k_vis_project<<<b2v_grid((int64_t)nviews * nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, nviews, w.cams, w.proj);
   if (int rc = b2v_check_launch("k_vis_project")) return rc;
-  k_vis_merge_insert<<<b2v_grid(nv, kBlock, 16), kBlock, 0, s>>>(verts, nv, w.hmask, w.slots, w.rep);
-  if (int rc = b2v_check_launch("k_vis_merge_insert")) return rc;
+  if (int rc = merge_points(verts, nv, w.hmask, w.slots, w.rep, s)) return rc;
   if (nt > 0) {
     k_vis_raster<<<b2v_grid((int64_t)nviews * nt, kBlock, 16), kBlock, 0, s>>>(F, nviews, w.proj, w.zbuf, w.queue,
                                                                                w.qcount, w.misc);
