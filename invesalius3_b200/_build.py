@@ -79,20 +79,12 @@ def build_cuda(force: bool = False, verbose: bool = False) -> Path:
 
 
 def build_oracle(force: bool = False) -> Path:
-    """Compile the CPU oracle (test infrastructure only) via oracle/Makefile, the 3-D mask
-    editor's checker via oracle/editor.mk, the jump-flooding checker via oracle/voronoi.mk, the
-    visible-faces checker via oracle/visibility.mk, the connectivity checker via
-    oracle/connectivity.mk, the smoothing checker via oracle/smoothing.mk, the hole-filling checker via
-    oracle/fill_holes.mk, the normals checker via oracle/normals.mk, the geodesic checker via oracle/geodesic.mk,
-    the volume rendering's data-preparation checker via oracle/raycasting.mk and the clean and triangle filter's
-    checker via oracle/clean.mk."""
-    for makefile in ([], ["-f", "editor.mk"], ["-f", "voronoi.mk"], ["-f", "visibility.mk"],
-                     ["-f", "connectivity.mk"], ["-f", "smoothing.mk"], ["-f", "fill_holes.mk"],
-                     ["-f", "normals.mk"], ["-f", "geodesic.mk"], ["-f", "raycasting.mk"], ["-f", "clean.mk"]):
-        r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *makefile, *(["-B"] if force else [])],
-                           capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"oracle build failed:\n{r.stdout}\n{r.stderr}")
+    """Compile the CPU oracle and its checkers (test infrastructure only) into oracle/liboracle.so
+    via oracle/Makefile."""
+    r = subprocess.run(["make", "-C", str(ROOT / "oracle"), *(["-B"] if force else [])],
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"oracle build failed:\n{r.stdout}\n{r.stderr}")
     return ROOT / "oracle" / "liboracle.so"
 
 

@@ -22,13 +22,12 @@ _LIB = None
 
 
 def lib() -> C.CDLL:
+    """liboracle.so, the one library of every C checker, loaded once per process. make decides whether it is
+    stale, so the rebuild follows oracle/Makefile's prerequisites exactly and does nothing when it is not."""
     global _LIB
     if _LIB is None:
-        so = _HERE / "liboracle.so"
-        srcs = list(_HERE.glob("*.c"))
-        if not so.exists() or any(so.stat().st_mtime < s.stat().st_mtime for s in srcs):
-            subprocess.run(["make", "-C", str(_HERE)], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
+        subprocess.run(["make", "-C", str(_HERE)], check=True, capture_output=True)
+        _LIB = C.CDLL(str(_HERE / "liboracle.so"))
     return _LIB
 
 
@@ -37,8 +36,22 @@ def _estrides(a: np.ndarray):
     return (C.c_int64 * a.ndim)(*[s // a.itemsize for s in a.strides])
 
 
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+def _ptr(a: np.ndarray | None):
+    return C.c_void_p(None if a is None else a.ctypes.data)
+
+
+def _faces3(faces) -> np.ndarray:
+    """Contiguous int64 [T,3] of int32 / int64 faces [T,3] or [T,4] with a leading 3 in every row."""
+    f = np.asarray(faces)
+    if f.dtype not in (np.int32, np.int64):
+        raise TypeError("faces: int32 or int64 expected")
+    if f.ndim != 2 or f.shape[1] not in (3, 4):
+        raise ValueError("faces: [T,3] or [T,4] expected")
+    if f.shape[1] == 4:
+        if len(f) and (f[:, 0] != 3).any():
+            raise ValueError("faces: the [T,4] form needs a leading 3 in every row")
+        f = f[:, 1:]
+    return np.ascontiguousarray(f, dtype=np.int64)
 
 
 _SUFFIX = {np.dtype(np.int16): "i16", np.dtype(np.uint8): "u8", np.dtype(np.float64): "f64"}

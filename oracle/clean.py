@@ -1,6 +1,6 @@
 """CPU checker of the surface clean and triangle filter — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/clean.c (built into oracle/libclean.so by oracle/clean.mk): sequential
+ctypes wrapper of oracle/clean.c (built into oracle/liboracle.so): sequential
 vtkCleanPolyData and vtkTriangleFilter on polys and strips. Inputs take the forms the product takes (faces
 [T,3] / [T,4] with a leading 3, or an (offsets, connectivity) pair); outputs are int64 cell arrays.
 PARITY WITH VTK UNPINNED: see clean.c's header.
@@ -8,27 +8,10 @@ PARITY WITH VTK UNPINNED: see clean.c's header.
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libclean.so", _HERE / "clean.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "clean.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+from oracle import _ptr, lib
 
 
 def cell_array(x):

@@ -1,6 +1,6 @@
 """CPU checker of the surface connectivity tools — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/connectivity.c (built into oracle/libconnectivity.so by oracle/connectivity.mk):
+ctypes wrapper of oracle/connectivity.c (built into oracle/liboracle.so):
 the traversal of vtkPolyDataConnectivityFilter, and the outputs of polydata_utils.SelectLargestPart,
 SplitDisconectedParts and JoinSeedsParts on arrays, assembled from it.
 PARITY WITH VTK UNPINNED: see connectivity.c's header and DESIGN.md §5.
@@ -8,40 +8,10 @@ PARITY WITH VTK UNPINNED: see connectivity.c's header and DESIGN.md §5.
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libconnectivity.so", _HERE / "connectivity.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "connectivity.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
-
-
-def _faces3(faces) -> np.ndarray:
-    f = np.asarray(faces)
-    if f.dtype not in (np.int32, np.int64):
-        raise TypeError("faces: int32 or int64 expected")
-    if f.ndim != 2 or f.shape[1] not in (3, 4):
-        raise ValueError("faces: [T,3] or [T,4] expected")
-    if f.shape[1] == 4:
-        if len(f) and (f[:, 0] != 3).any():
-            raise ValueError("faces: the [T,4] form needs a leading 3 in every row")
-        f = f[:, 1:]
-    return np.ascontiguousarray(f, dtype=np.int64)
+from oracle import _faces3, _ptr, lib
 
 
 def traverse(nv: int, faces, seeds=None) -> dict:

@@ -1,39 +1,18 @@
 """CPU checker for the 3-D mask editor — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrappers of oracle/editor.c (built into oracle/libeditor.so by oracle/editor.mk) with the
+ctypes wrappers of oracle/editor.c (built into oracle/liboracle.so) with the
 crate's names and argument order (invesalius_rs.polygon2mask_rs, mask_cut, brush_mask_rs), so the
 parity tests read like calls of the reference. PARITY UNPINNED: see editor.c's header and DESIGN.md §5.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
+from oracle import _estrides, _ptr, lib
+
 _IMAGE_DTYPES = (np.dtype(np.int16), np.dtype(np.uint8), np.dtype(np.float64))
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libeditor.so", _HERE / "editor.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "editor.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _estrides(a: np.ndarray):
-    assert all(s % a.itemsize == 0 for s in a.strides)
-    return (C.c_int64 * a.ndim)(*[s // a.itemsize for s in a.strides])
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
 
 
 def polygon2mask_rs(shape, polygon):

@@ -1,38 +1,20 @@
 """CPU checker of the surface hole filler — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/fill_holes.c (built into oracle/libfill_holes.so by oracle/fill_holes.mk): the
+ctypes wrapper of oracle/fill_holes.c (built into oracle/liboracle.so): the
 sequential vtkFillHolesFilter, with its boundary lines and per-loop records.
 PARITY WITH VTK UNPINNED: see fill_holes.c's header and DESIGN.md §5.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-from oracle.connectivity import _faces3
+from oracle import _faces3, _ptr, lib
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
 
 FILLED, FAILED, TOO_LARGE = 0, 1, 2
 FLT_MAX = float(np.finfo(np.float32).max)
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libfill_holes.so", _HERE / "fill_holes.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "fill_holes.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
 
 
 def fill_holes(vertices, faces, hole_size=1.0) -> dict:

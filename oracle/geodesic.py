@@ -1,6 +1,6 @@
 """CPU checker of the geodesic surface measurement — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/geodesic.c (built into oracle/libgeodesic.so by oracle/geodesic.mk): the closest points
+ctypes wrapper of oracle/geodesic.c (built into oracle/liboracle.so): the closest points
 of vtkPointLocator, the sequential vtkDijkstraGraphGeodesicPath (distances, heap predecessors and trace), the
 per-point ambiguity and the device's predecessor rule, and the path length as measures.py sums it.
 PARITY WITH VTK UNPINNED: see geodesic.c's header and DESIGN.md.
@@ -8,30 +8,10 @@ PARITY WITH VTK UNPINNED: see geodesic.c's header and DESIGN.md.
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-from oracle.connectivity import _faces3
-
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libgeodesic.so", _HERE / "geodesic.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "geodesic.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-        _LIB.orc_geodesic_trace.restype = C.c_int64
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+from oracle import _faces3, _ptr, lib
 
 
 def _points(vertices) -> np.ndarray:
@@ -57,8 +37,9 @@ def trace(pre: np.ndarray, start: int, end: int) -> np.ndarray:
     """TraceShortestPath over `pre`: int64 ids from the end to the start (the end alone when unreached)."""
     pre = np.ascontiguousarray(pre, dtype=np.int64)
     ids = np.empty(len(pre), np.int64)
-    n = lib().orc_geodesic_trace(_ptr(pre), C.c_int64(len(pre)), C.c_int64(int(start)), C.c_int64(int(end)),
-                                 _ptr(ids))
+    fn = lib().orc_geodesic_trace
+    fn.restype = C.c_int64
+    n = fn(_ptr(pre), C.c_int64(len(pre)), C.c_int64(int(start)), C.c_int64(int(end)), _ptr(ids))
     if n < 0:
         raise ValueError("geodesic trace: the predecessors form a cycle")
     return ids[:n].copy()

@@ -1,6 +1,6 @@
 """CPU checker of surface normals and mass properties — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/normals.c (built into oracle/libnormals.so by oracle/normals.mk): the sequential
+ctypes wrapper of oracle/normals.c (built into oracle/liboracle.so): the sequential
 vtkPolyDataNormals (consistent order, auto-orientation, feature splitting, cell and point normals) and
 vtkMassProperties' volume and area.
 PARITY WITH VTK UNPINNED: see normals.c's header and DESIGN.md §5.
@@ -8,29 +8,10 @@ PARITY WITH VTK UNPINNED: see normals.c's header and DESIGN.md §5.
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-from oracle.connectivity import _faces3
-
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libnormals.so", _HERE / "normals.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "normals.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+from oracle import _faces3, _ptr, lib
 
 
 def compute_normals(vertices, faces, feature_angle=30.0, auto_orient=False) -> dict:

@@ -1,33 +1,16 @@
 """CPU checker of the volume rendering's data preparation — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/raycasting.c (built into oracle/libraycasting.so by oracle/raycasting.mk): the flip and
+ctypes wrapper of oracle/raycasting.c (built into oracle/liboracle.so): the flip and
 unsigned-short shift of Volume.LoadVolume, the preset convolutions of ApplyConvolution and the histogram of
 CalculateHistogram (invesalius/data/volume.py). PARITY WITH VTK UNPINNED: see raycasting.c's header.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libraycasting.so", _HERE / "raycasting.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "raycasting.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+from oracle import _ptr, lib
 
 
 def _volume(matrix, dtype) -> np.ndarray:

@@ -1,6 +1,6 @@
 """CPU checker of the Laplacian surface smoothing — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/smoothing.c (built into oracle/libsmoothing.so by oracle/smoothing.mk): the
+ctypes wrapper of oracle/smoothing.c (built into oracle/liboracle.so): the
 sequential vtkSmoothPolyDataFilter, with its point types and edge lists.
 PARITY WITH VTK UNPINNED: see smoothing.c's header and DESIGN.md §5.
 """
@@ -8,29 +8,10 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-from oracle.connectivity import _faces3
-
-_HERE = Path(__file__).resolve().parent
-_LIB = None
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libsmoothing.so", _HERE / "smoothing.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "smoothing.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray):
-    return C.c_void_p(a.ctypes.data)
+from oracle import _faces3, _ptr, lib
 
 
 def cosine(angle: float) -> float:

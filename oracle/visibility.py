@@ -1,37 +1,21 @@
 """CPU checker for "Remove non-visible faces" — TEST INFRASTRUCTURE ONLY.
 
-ctypes wrapper of oracle/visibility.c (built into oracle/libvisibility.so by oracle/visibility.mk) with the
+ctypes wrapper of oracle/visibility.c (built into oracle/liboracle.so) with the
 plugin's signature on arrays: remove_non_visible_faces(vertices, faces, positions, remove_visible).
 PARITY WITH VTK UNPINNED: see visibility.c's header and DESIGN.md §5.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
+from oracle import _faces3, _ptr, lib
+
 RES = 800
 CAMERA_DOUBLES = 32
 BIG_BOX = 64
 DEFAULT_POSITIONS = ((1, 0, 0), (-1, 0, 0), (0, 1, 0), (0, -1, 0), (0, 0, 1), (0, 0, -1))
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libvisibility.so", _HERE / "visibility.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "visibility.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
-
-
-def _ptr(a: np.ndarray | None):
-    return C.c_void_p(None if a is None else a.ctypes.data)
 
 
 def _positions(positions) -> np.ndarray:
@@ -62,22 +46,6 @@ def cameras(bnds, positions=DEFAULT_POSITIONS) -> np.ndarray:
     return out
 
 
-def _faces3(faces: np.ndarray, nv: int) -> np.ndarray:
-    f = np.asarray(faces)
-    if f.dtype not in (np.int32, np.int64):
-        raise TypeError("faces: int32 or int64 expected")
-    if f.ndim != 2 or f.shape[1] not in (3, 4):
-        raise ValueError("faces: [T,3] or [T,4] expected")
-    if f.shape[1] == 4:
-        if len(f) and (f[:, 0] != 3).any():
-            raise ValueError("faces: the [T,4] form needs a leading 3 in every row")
-        f = f[:, 1:]
-    f = np.ascontiguousarray(f, dtype=np.int64)
-    if len(f) and (f.min() < 0 or f.max() >= nv):
-        raise ValueError("faces: index out of range")
-    return f
-
-
 def remove_non_visible_faces(vertices, faces, positions=DEFAULT_POSITIONS, remove_visible=False, debug=False):
     """(vertices float32 [V',3], faces int32 [T',3]); with debug=True also a dict with the cameras, the
     depth buffers float64 [views][800][800], the per-vertex visibility and the count of triangles whose
@@ -90,7 +58,9 @@ def remove_non_visible_faces(vertices, faces, positions=DEFAULT_POSITIONS, remov
     if not np.isfinite(v).all():
         raise ValueError("vertices must be finite")
     v = np.ascontiguousarray(v)
-    f = _faces3(faces, len(v))
+    f = _faces3(faces)
+    if len(f) and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError("faces: index out of range")
     p = _positions(positions)
     nv, nt, nviews = len(v), len(f), len(p)
     cams = np.zeros((nviews, CAMERA_DOUBLES), np.float64)

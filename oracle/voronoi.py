@@ -1,6 +1,6 @@
 """CPU checker for the porous-scaffold Voronoi generator — TEST INFRASTRUCTURE ONLY.
 
-jump_flooding: ctypes wrapper of oracle/voronoi.c (built into oracle/libvoronoi.so by oracle/voronoi.mk) with
+jump_flooding: ctypes wrapper of oracle/voronoi.c (built into oracle/liboracle.so) with
 the crate's name and argument order (invesalius_rs.jump_flooding, in place). create_voronoi,
 create_voronoi_non_random and image_normalize restate plugins/porous_creation/schwarzp.py:37-84 and
 imagedata_utils.py:580-587 in NumPy / SciPy: the checker's jump_flooding, then np.gradient,
@@ -12,25 +12,13 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import subprocess
-from pathlib import Path
 
 import numpy as np
 from scipy import ndimage as ndi
 
-_HERE = Path(__file__).resolve().parent
-_LIB = None
+from oracle import _ptr, lib
+
 GAUSSIAN_SIGMA = 1.5
-
-
-def lib() -> C.CDLL:
-    global _LIB
-    if _LIB is None:
-        so, src = _HERE / "libvoronoi.so", _HERE / "voronoi.c"
-        if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-            subprocess.run(["make", "-C", str(_HERE), "-f", "voronoi.mk"], check=True, capture_output=True)
-        _LIB = C.CDLL(str(so))
-    return _LIB
 
 
 def jump_flooding(distance_map, map_owners, sites, normalize, nthreads=None):
@@ -49,9 +37,8 @@ def jump_flooding(distance_map, map_owners, sites, normalize, nthreads=None):
     o = np.ascontiguousarray(map_owners)
     s = np.ascontiguousarray(sites[:, :3])
     nthreads = nthreads or os.cpu_count() or 1
-    lib().orc_jump_flooding(C.c_void_p(d.ctypes.data), C.c_void_p(o.ctypes.data), *map(C.c_int64, d.shape),
-                            C.c_void_p(s.ctypes.data), C.c_int64(len(s)), C.c_int(int(bool(normalize))),
-                            C.c_int(int(nthreads)))
+    lib().orc_jump_flooding(_ptr(d), _ptr(o), *map(C.c_int64, d.shape), _ptr(s), C.c_int64(len(s)),
+                            C.c_int(int(bool(normalize))), C.c_int(int(nthreads)))
     distance_map[...] = d
     map_owners[...] = o
 
