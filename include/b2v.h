@@ -34,6 +34,9 @@ extern "C" {
 #define B2V_I16 0
 #define B2V_U8 1
 #define B2V_F64 2
+/* B2V_F32 (3) is defined with b2v_zoom below; label images of count_regions also come as int32 / int64 */
+#define B2V_I32 4
+#define B2V_I64 5
 
 /* projection kinds for b2v_mip */
 #define B2V_MIP_MAX 0
@@ -257,13 +260,40 @@ int b2v_histogram_i16(const int16_t* a, int64_t n, int lo, int bins, int64_t* co
  * too); labels uint32, numbered in raster order of each component's first voxel like SciPy.
  * *nlabels_host receives the count. SYNCHRONISES. workspace: b2v_label_workspace_bytes(n voxels).
  * b2v_count_regions: invesalius_rs.count_regions (count_regions.rs:5-18): out[p] = number of voxels
- * holding image[p]'s value; values outside [0, number_regions] are B2V_ERR_RANGE (the reference
- * panics). workspace: 256 + 4 * (number_regions + 1) bytes. */
+ * holding image[p]'s value; image dtype B2V_I16, B2V_U8, B2V_I32 or B2V_I64 (else B2V_ERR_ARG); values
+ * outside [0, number_regions] are B2V_ERR_RANGE (the reference panics). SYNCHRONISES. workspace:
+ * 256 + 4 * (number_regions + 1) bytes.
+ * b2v_region_sizes: the size table of count_regions alone: sizes[v] = number of voxels holding v, for v in
+ * [0, number_regions] (device uint32 [number_regions + 1]); same dtypes and errors. SYNCHRONISES.
+ * workspace: 256 bytes.
+ * Both add each run of equal values a warp reads with one atomic, so a dominant label (the background)
+ * does not serialise the count. 64-bit indexing: n may exceed 2^31. */
 int64_t b2v_label_workspace_bytes(int64_t n);
 int b2v_label(const uint8_t* input, int64_t nz, int64_t ny, int64_t nx, const uint8_t* strct_host, int64_t odz, int64_t ody,
               int64_t odx, uint32_t* labels, void* workspace, void* stream, int64_t* nlabels_host);
 int b2v_count_regions(const void* image, int dtype, int64_t n, uint32_t number_regions, uint32_t* out, void* workspace,
                       void* stream);
+int b2v_region_sizes(const void* image, int dtype, int64_t n, uint32_t number_regions, uint32_t* sizes, void* workspace,
+                     void* stream);
+
+/* The "Remove tiny objects" plugin (plugins/remove_tiny_objects/gui.py:36-62, 134-144) over a resident label
+ * image: labels uint32 [dz][dy][dx] (b2v_label's output) and its size table sizes uint32 [nsizes]
+ * (b2v_region_sizes). A voxel is tiny where sizes[labels[p]] <= min_size, compared exactly as int64 (a
+ * negative min_size selects nothing); a label >= nsizes is never tiny. nsizes: 0 .. 2^32. None of the three
+ * synchronises; all index in 64 bits.
+ *   b2v_tiny_objects_preview        out[p] = tiny ? 255 : 0, out dense uint8 [n] (the plugin's preview,
+ *                                   `(counts <= min_size) * 255`). 4 B read + 1 B written per voxel.
+ *   b2v_tiny_objects_remove         mask[1 + z][1 + y][1 + x] = 1 where (z, y, x) is tiny, on the padded
+ *                                   uint8 [dz + 1][dy + 1][dx + 1] mask layout, in place; the flag planes
+ *                                   (z = 0, y = 0, x = 0) and the other body voxels are not written.
+ *   b2v_tiny_objects_apply_preview  the same write where preview[p] > 127, preview dense uint8 [dz][dy][dx]
+ *                                   (OnRemove's `m[preview > 127] = 1`). */
+int b2v_tiny_objects_preview(const uint32_t* labels, int64_t n, const uint32_t* sizes, int64_t nsizes, int64_t min_size,
+                             uint8_t* out, void* stream);
+int b2v_tiny_objects_remove(const uint32_t* labels, int64_t dz, int64_t dy, int64_t dx, const uint32_t* sizes,
+                            int64_t nsizes, int64_t min_size, uint8_t* mask, void* stream);
+int b2v_tiny_objects_apply_preview(const uint8_t* preview, int64_t dz, int64_t dy, int64_t dx, uint8_t* mask,
+                                   void* stream);
 
 /* Labelling of a Z-sharded volume (dist.label): every shard labels its own planes with b2v_label
  * (local labels 1..n_r); the provisional id of local label l on shard r is P = base_r + l, base_r the

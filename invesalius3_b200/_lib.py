@@ -68,6 +68,10 @@ PROTOTYPES = {
     "b2v_label_workspace_bytes": (i64, [i64]),
     "b2v_label": (cint, [vp, i64, i64, i64, vp, i64, i64, i64, vp, vp, vp, C.POINTER(i64)]),
     "b2v_count_regions": (cint, [vp, cint, i64, u32, vp, vp, vp]),
+    "b2v_region_sizes": (cint, [vp, cint, i64, u32, vp, vp, vp]),
+    "b2v_tiny_objects_preview": (cint, [vp, i64, vp, i64, i64, vp, vp]),
+    "b2v_tiny_objects_remove": (cint, [vp, i64, i64, i64, vp, i64, i64, vp, vp]),
+    "b2v_tiny_objects_apply_preview": (cint, [vp, i64, i64, i64, vp, vp]),
     "b2v_label_boundary_workspace_bytes": (i64, [i64, i64, i64, i64]),
     "b2v_label_boundary_count": (cint, [vp, vp, i64, i64, vp, i64, i64, i64, i64, i64, vp, vp, C.POINTER(i64)]),
     "b2v_label_boundary_emit": (cint, [vp, vp, i64, i64, i64, i64, i64, i64, vp, vp, vp]),
@@ -175,6 +179,7 @@ PROTOTYPES = {
 VIS_CAMERA_DOUBLES = 32
 
 F32 = 3
+I32, I64 = 4, 5
 ZOOM_CONSTANT, ZOOM_MIRROR = 0, 1
 
 SEL_EQ, SEL_GT127 = 0, 1

@@ -12,6 +12,8 @@
 #include "b2v_common.cuh"
 #include "scan.cuh"
 
+#include <type_traits>
+
 namespace {
 
 __device__ __forceinline__ int uf_find(int* p, int i) {
@@ -132,16 +134,59 @@ __global__ void __launch_bounds__(256) k_label_assign(const int* __restrict__ pa
   }
 }
 
-// count_regions (count_regions.rs:5-18): out[p] = number of voxels that carry image[p]'s value
-template <typename T>
-__global__ void __launch_bounds__(256) k_count_hist(const T* __restrict__ img, long long n, uint32_t nbins, uint32_t* counts,
-                                                    int* status) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long v = (long long)img[i];
-    if (v < 0 || v >= (long long)nbins) { *status = 1; continue; }
-    atomicAdd(&counts[v], 1u);
+// count_regions (count_regions.rs:5-18): out[p] = number of voxels that carry image[p]'s value.
+// The size table is a histogram whose background bin usually holds most of the volume, so one atomic per
+// voxel would serialise on it. Each lane keeps the run of equal values it is reading (value, length) and
+// only adds a run to the table where its value changes; the lanes of a warp that end runs of one value at
+// the same step add them with one atomic. A volume of one label costs one atomic per warp.
+// All lanes of a warp call this together (f: this lane ends the run v of length c). The lanes that end runs
+// of one value at one step are neighbours (they crossed the same edge); where no two neighbours do, as in
+// noise, the grouping would buy nothing and each lane adds its own run.
+__device__ __forceinline__ void add_runs(bool f, uint32_t v, uint32_t c, uint32_t* counts) {
+  const unsigned any = __ballot_sync(0xffffffffu, f);
+  if (!any) return;
+  const uint32_t next = __shfl_down_sync(0xffffffffu, v, 1);
+  const unsigned pairs = __ballot_sync(0xffffffffu, f && v == next) & (any >> 1);
+  if (!f) return;
+  if (!pairs) {
+    atomicAdd(&counts[v], c);
+    return;
   }
+  const unsigned g = __match_any_sync(any, v);
+  const unsigned s = __reduce_add_sync(g, c);
+  if ((threadIdx.x & 31) == (unsigned)(__ffs(g) - 1)) atomicAdd(&counts[v], s);
+}
+
+// counts[v] += voxels holding v, v in [0, nbins); any other value sets *status. The trip count depends on
+// the warp only, so every warp stays converged for add_runs (block size: a multiple of 32).
+template <typename T>
+__global__ void __launch_bounds__(256) k_region_sizes(const T* __restrict__ img, int64_t n, uint32_t nbins,
+                                                      uint32_t* counts, int* status) {
+  constexpr int U = 8;                       // loads in flight per lane
+  const unsigned lane = threadIdx.x & 31;
+  const int64_t step = gstride() * U;
+  uint32_t cv = 0, cc = 0;                   // this lane's run: value, length (0: none yet)
+  for (int64_t base = (gtid() - lane) * U; base < n; base += step) {
+    T v[U];
+#pragma unroll
+    for (int k = 0; k < U; ++k) {
+      const int64_t i = base + k * 32 + lane;
+      v[k] = i < n ? img[i] : T(0);
+    }
+#pragma unroll
+    for (int k = 0; k < U; ++k) {
+      const int64_t x = (int64_t)v[k];
+      const bool in = base + k * 32 + lane < n;
+      const bool ok = in && x >= 0 && x < (int64_t)nbins;
+      if (in && !ok) *status = 1;
+      add_runs(ok && cc && (uint32_t)x != cv, cv, cc, counts);
+      if (ok) {
+        cc = (cc && (uint32_t)x == cv) ? cc + 1 : 1;
+        cv = (uint32_t)x;
+      }
+    }
+  }
+  add_runs(cc != 0, cv, cc, counts);
 }
 template <typename T>
 __global__ void __launch_bounds__(256) k_count_gather(const T* __restrict__ img, long long n, uint32_t nbins,
@@ -150,6 +195,46 @@ __global__ void __launch_bounds__(256) k_count_gather(const T* __restrict__ img,
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const long long v = (long long)img[i];
     out[i] = (v >= 0 && v < (long long)nbins) ? counts[v] : 0u;
+  }
+}
+
+// ---- the remove-tiny-objects plugin (plugins/remove_tiny_objects/gui.py) over a resident label image ----
+// A voxel is tiny where its region holds at most min_size voxels (labels outside the size table never are).
+struct TinyRegion {
+  const uint32_t* __restrict__ labels;
+  const uint32_t* __restrict__ sizes;
+  int64_t nsizes;
+  int64_t min_size;
+  __device__ __forceinline__ bool of(uint32_t l) const { return l < nsizes && (int64_t)__ldg(sizes + l) <= min_size; }
+  __device__ __forceinline__ bool operator()(int64_t i) const { return of(labels[i]); }
+};
+
+// The plugin's OnRemove selection: preview > 127.
+struct PreviewSet {
+  const uint8_t* __restrict__ preview;
+  __device__ __forceinline__ bool operator()(int64_t i) const { return preview[i] > 127; }
+};
+
+// out[i] = 255 where tiny, else 0; vec: labels 16-byte and out 4-byte aligned, four voxels a lane
+__global__ void __launch_bounds__(256) k_tiny_preview(TinyRegion t, int64_t n, uint8_t* __restrict__ out, bool vec) {
+  const int64_t nv = vec ? n / 4 : 0;
+  for (int64_t j = gtid(); j < nv; j += gstride()) {
+    const uint4 l = reinterpret_cast<const uint4*>(t.labels)[j];
+    reinterpret_cast<uint32_t*>(out)[j] = (t.of(l.x) ? 0xffu : 0u) | (t.of(l.y) ? 0xff00u : 0u) |
+                                          (t.of(l.z) ? 0xff0000u : 0u) | (t.of(l.w) ? 0xff000000u : 0u);
+  }
+  for (int64_t i = nv * 4 + gtid(); i < n; i += gstride()) out[i] = t(i) ? 255 : 0;
+}
+
+// mask[1 + z][1 + y][1 + x] = 1 where sel(body index), on the padded [dz + 1][dy + 1][dx + 1] layout; the
+// flag planes z = 0, y = 0 and x = 0 are never written. One block a body row.
+template <class Sel>
+__global__ void __launch_bounds__(256) k_mark_body(Sel sel, int64_t dy, int64_t dx, int64_t nrows, uint8_t* mask) {
+  for (int64_t r = blockIdx.x; r < nrows; r += gridDim.x) {
+    const int64_t z = r / dy, y = r - z * dy;
+    uint8_t* row = mask + ((z + 1) * (dy + 1) + y + 1) * (dx + 1) + 1;
+    for (int64_t x = threadIdx.x; x < dx; x += blockDim.x)
+      if (sel(r * dx + x)) row[x] = 1;
   }
 }
 
@@ -530,6 +615,48 @@ extern "C" int b2v_label_relabel(uint32_t* labels, int64_t n, const uint32_t* lu
   return b2v_check_launch("k_label_relabel");
 }
 
+// f((const T*)image) for the label dtypes of count_regions; B2V_ERR_ARG for any other
+template <class F>
+static int with_label_type(const void* image, int dtype, F&& f) {
+  switch (dtype) {
+    case B2V_I16: return f((const int16_t*)image);
+    case B2V_U8: return f((const uint8_t*)image);
+    case B2V_I32: return f((const int32_t*)image);
+    case B2V_I64: return f((const int64_t*)image);
+  }
+  B2V_REQUIRE(false, B2V_ERR_ARG, "count_regions: image must be int16, int32, int64 or uint8");
+}
+
+// sizes[0, nbins) = the histogram of image; status (device int) set where a value lies outside it. Enqueues only.
+static int region_sizes(const void* image, int dtype, int64_t n, uint32_t nbins, uint32_t* sizes, int* status,
+                        cudaStream_t s) {
+  B2V_CUDA(cudaMemsetAsync(status, 0, sizeof(int), s));
+  B2V_CUDA(cudaMemsetAsync(sizes, 0, (size_t)nbins * 4, s));
+  const int rc = with_label_type(image, dtype, [&](auto img) {
+    using T = std::remove_const_t<std::remove_pointer_t<decltype(img)>>;
+    k_region_sizes<T><<<b2v_grid(n, 256 * 8, 16), 256, 0, s>>>(img, n, nbins, sizes, status);
+    return b2v_check_launch("k_region_sizes");
+  });
+  return rc;
+}
+
+static int range_status(const int* status, cudaStream_t s) {
+  int st = 0;
+  B2V_CUDA(cudaMemcpyAsync(&st, status, sizeof(int), cudaMemcpyDeviceToHost, s));
+  B2V_CUDA(cudaStreamSynchronize(s));
+  B2V_REQUIRE(st == 0, B2V_ERR_RANGE, "count_regions: a value lies outside [0, number_regions] (the reference panics here)");
+  return B2V_OK;
+}
+
+extern "C" int b2v_region_sizes(const void* image, int dtype, int64_t n, uint32_t number_regions, uint32_t* sizes,
+                                void* workspace, void* stream) {
+  B2V_REQUIRE(image && sizes && workspace && n > 0, B2V_ERR_ARG, "region_sizes: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  int rc;
+  if ((rc = region_sizes(image, dtype, n, number_regions + 1, sizes, (int*)workspace, s))) return rc;
+  return range_status((const int*)workspace, s);
+}
+
 extern "C" int b2v_count_regions(const void* image, int dtype, int64_t n, uint32_t number_regions, uint32_t* out,
                                  void* workspace, void* stream) {
   B2V_REQUIRE(image && out && workspace && n > 0, B2V_ERR_ARG, "count_regions: bad arguments");
@@ -537,23 +664,54 @@ extern "C" int b2v_count_regions(const void* image, int dtype, int64_t n, uint32
   const uint32_t nbins = number_regions + 1;
   int* status = (int*)workspace;
   uint32_t* counts = (uint32_t*)((char*)workspace + 256);
-  B2V_CUDA(cudaMemsetAsync(workspace, 0, 256 + (size_t)nbins * 4, s));
   int rc;
-  if (dtype == B2V_I16) {
-    k_count_hist<int16_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, status);
-    if ((rc = b2v_check_launch("k_count_hist"))) return rc;
-    k_count_gather<int16_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const int16_t*)image, n, nbins, counts, out);
-  } else if (dtype == B2V_U8) {
-    k_count_hist<uint8_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, status);
-    if ((rc = b2v_check_launch("k_count_hist"))) return rc;
-    k_count_gather<uint8_t><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>((const uint8_t*)image, n, nbins, counts, out);
-  } else {
-    B2V_REQUIRE(false, B2V_ERR_ARG, "count_regions: image must be int16 or uint8");
-  }
-  if ((rc = b2v_check_launch("k_count_gather"))) return rc;
-  int st = 0;
-  B2V_CUDA(cudaMemcpyAsync(&st, status, sizeof(int), cudaMemcpyDeviceToHost, s));
-  B2V_CUDA(cudaStreamSynchronize(s));
-  B2V_REQUIRE(st == 0, B2V_ERR_RANGE, "count_regions: a value lies outside [0, number_regions] (the reference panics here)");
+  if ((rc = region_sizes(image, dtype, n, nbins, counts, status, s))) return rc;
+  rc = with_label_type(image, dtype, [&](auto img) {
+    using T = std::remove_const_t<std::remove_pointer_t<decltype(img)>>;
+    k_count_gather<T><<<b2v_grid(n, 256 * 4, 16), 256, 0, s>>>(img, n, nbins, counts, out);
+    return b2v_check_launch("k_count_gather");
+  });
+  if (rc) return rc;
+  return range_status(status, s);
+}
+
+static int tiny_check(const void* in, const uint32_t* sizes, int64_t nsizes, const void* out) {
+  B2V_REQUIRE(in && out && (sizes || !nsizes), B2V_ERR_ARG, "tiny_objects: null pointer");
+  B2V_REQUIRE(nsizes >= 0 && nsizes <= (1ll << 32), B2V_ERR_ARG, "tiny_objects: the size table holds 0 .. 2^32 entries");
   return B2V_OK;
+}
+
+extern "C" int b2v_tiny_objects_preview(const uint32_t* labels, int64_t n, const uint32_t* sizes, int64_t nsizes,
+                                        int64_t min_size, uint8_t* out, void* stream) {
+  int rc;
+  if ((rc = tiny_check(labels, sizes, nsizes, out))) return rc;
+  B2V_REQUIRE(n >= 0, B2V_ERR_ARG, "tiny_objects_preview: negative voxel count");
+  if (!n) return B2V_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  const bool vec = b2v_aligned16(labels) && ((uintptr_t)out & 3u) == 0;
+  k_tiny_preview<<<b2v_grid(n, 256 * 16, 16), 256, 0, s>>>(TinyRegion{labels, sizes, nsizes, min_size}, n, out, vec);
+  return b2v_check_launch("k_tiny_preview");
+}
+
+template <class Sel>
+static int mark_body(Sel sel, int64_t dz, int64_t dy, int64_t dx, uint8_t* mask, cudaStream_t s) {
+  B2V_REQUIRE(dz >= 0 && dy >= 0 && dx >= 0, B2V_ERR_ARG, "tiny_objects: negative body shape");
+  const int64_t nrows = dz * dy;
+  if (!nrows || !dx) return B2V_OK;
+  k_mark_body<<<b2v_grid(nrows, 1, 16), 256, 0, s>>>(sel, dy, dx, nrows, mask);
+  return b2v_check_launch("k_mark_body");
+}
+
+extern "C" int b2v_tiny_objects_remove(const uint32_t* labels, int64_t dz, int64_t dy, int64_t dx, const uint32_t* sizes,
+                                       int64_t nsizes, int64_t min_size, uint8_t* mask, void* stream) {
+  int rc;
+  if ((rc = tiny_check(labels, sizes, nsizes, mask))) return rc;
+  return mark_body(TinyRegion{labels, sizes, nsizes, min_size}, dz, dy, dx, mask, (cudaStream_t)stream);
+}
+
+extern "C" int b2v_tiny_objects_apply_preview(const uint8_t* preview, int64_t dz, int64_t dy, int64_t dx, uint8_t* mask,
+                                              void* stream) {
+  int rc;
+  if ((rc = tiny_check(preview, nullptr, 0, mask))) return rc;
+  return mark_body(PreviewSet{preview}, dz, dy, dx, mask, (cudaStream_t)stream);
 }

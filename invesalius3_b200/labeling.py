@@ -2,6 +2,7 @@
 
   label(input, structure, output=np.uint32)     scipy.ndimage.label   mask.py:526-530, 549-552
   count_regions(image, number_regions)          invesalius_rs.count_regions   count_regions.rs:5-18
+                                                (int16, int32, int64 or uint8 labels)
   get_largest_connected_component(image)        imagedata_utils.py:717-721
   fill_holes_auto(matrix, conn, size)           the body of Mask.fill_holes_auto (mask.py:519-562):
                                                 labelling and filling without leaving the device
@@ -66,16 +67,47 @@ def label(input, structure=None, output=np.uint32):
     return res.reshape(a.shape).astype(output, copy=False), n
 
 
-def count_regions(image: np.ndarray, number_regions: int) -> np.ndarray:
-    """invesalius_rs.count_regions (invesalius_rs/__init__.py:108-111): uint32 image of region sizes."""
-    a = np.asarray(image)
-    if a.dtype not in (np.int16, np.uint8) or a.ndim != 3:
-        raise TypeError("count_regions: int16 or uint8 3-D image expected")
-    t = dev.to_device(a)
+# label images count_regions takes: the crate's int16 / int32 / int64 (nd.label returns int32) and uint8
+_LABEL_DT = {torch.int16: _lib.I16, torch.uint8: _lib.U8, torch.int32: _lib.I32, torch.int64: _lib.I64}
+
+
+def _label_code(t: torch.Tensor) -> int:
+    _dense(t, "image")
+    try:
+        return _LABEL_DT[t.dtype]
+    except KeyError:
+        raise TypeError("count_regions: int16, int32, int64 or uint8 image expected") from None
+
+
+def count_regions_device(t: torch.Tensor, number_regions: int) -> torch.Tensor:
+    """count_regions on a dense device label image: an int32 tensor holding the uint32 region sizes.
+    A value outside [0, number_regions] raises ValueError. Synchronises."""
+    code = _label_code(t)
     out = torch.empty(t.shape, dtype=torch.int32, device=t.device)
     ws = _workspace(256 + 4 * (int(number_regions) + 1), t.device)
     with torch.cuda.device(t.device):
-        _lib.call("b2v_count_regions", _p(t), dev.dtype_code(t), t.numel(), int(number_regions), _p(out), _p(ws), _stream())
+        _lib.call("b2v_count_regions", _p(t), code, t.numel(), int(number_regions), _p(out), _p(ws), _stream())
+    return out
+
+
+def region_sizes_device(t: torch.Tensor, number_regions: int) -> torch.Tensor:
+    """The size table of count_regions: an int32 tensor [number_regions + 1] holding the uint32 number of
+    voxels of each value. A value outside [0, number_regions] raises ValueError. Synchronises."""
+    code = _label_code(t)
+    sizes = torch.empty(int(number_regions) + 1, dtype=torch.int32, device=t.device)
+    ws = _workspace(256, t.device)
+    with torch.cuda.device(t.device):
+        _lib.call("b2v_region_sizes", _p(t), code, t.numel(), int(number_regions), _p(sizes), _p(ws), _stream())
+    return sizes
+
+
+def count_regions(image: np.ndarray, number_regions: int) -> np.ndarray:
+    """invesalius_rs.count_regions (invesalius_rs/__init__.py:108-111): uint32 image of region sizes, for
+    int16, int32, int64 or uint8 labels."""
+    a = np.asarray(image)
+    if a.dtype not in (np.int16, np.int32, np.int64, np.uint8) or a.ndim != 3:
+        raise TypeError("count_regions: int16, int32, int64 or uint8 3-D image expected")
+    out = count_regions_device(dev.to_device(a), number_regions)
     res = np.empty(a.shape, np.uint32)
     dev.to_host(out, res.view(np.int32))
     return res
