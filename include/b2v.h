@@ -482,6 +482,43 @@ int b2v_voronoi_borders(const int32_t* owners, int64_t dz, int64_t dy, int64_t d
 int b2v_image_normalize_f32_i16(const float* in, int64_t n, float imin, float imax, float span, float min_f,
                                 int16_t fill, int16_t* out, void* stream);
 
+/* ---- porous scaffolds: TPMS and Blobs ---------------------------------------------------------------
+ * The other scaffolds of the porous-creation plugin (plugins/porous_creation/schwarzp.py:11-34, gui.py:117-245).
+ * surface: the triply periodic minimal surfaces in the plugin's combo order (B2V_TPMS_*). tables: dense float64
+ *   [cos_x (nx) | sin_x (nx) | cos_y (ny) | sin_y (ny) | cos_z (nz) | sin_z (nz)] on the device, NumPy's cos / sin
+ *   of the np.ogrid axes. Per voxel (z, y, x), with cx = cos_x[x], snx = sin_x[x] and so on, each product and sum
+ *   rounded on its own in this order (NumPy's broadcast evaluation of create_schwarzp, bit for bit):
+ *     P           (cx + cy) + cz
+ *     D           (((snx sny) snz + (snx cy) cz) + (cx sny) cz) + (cx cy) snz
+ *     Gyroid      (cx sny + cy snz) + cz snx
+ *     Neovius     3 ((cx + cy) + cz) + ((4 cx) cy) cz
+ *     iWP         ((cx cy + cy cz) + cz cx) - (cx cy) cz
+ *     P_W_Hybrid  (4 ((cx cy + cy cz) + cz cx) - ((3 cx) cy) cz) + 2.4
+ * b2v_tpms_f64: the float64 field into dense out [nz][ny][nx]. 8 B written per voxel.
+ * b2v_tpms_i16: image_normalize(field, min_, max_) into dense int16 out, without storing the field: one launch
+ *   evaluates it and reduces it to (imin, imax) (NaN-propagating, as NumPy's min / max), a second evaluates it
+ *   again and stores the C cast of (v - imin) * (span / (imax - imin)) + min_f in float64, or `fill` everywhere
+ *   when imin == imax. span = float64(max_ - min_), min_f = float64(min_). workspace:
+ *   b2v_tpms_i16_workspace_bytes; after the call its first 16 bytes hold (imin, imax) as float64. 2 B written per
+ *   voxel.
+ * b2v_image_normalize_f64_i16: the same two passes over a dense float64 device array of n elements
+ *   (imagedata_utils.py:580-587 for a float64 image): 2 x 8 B read + 2 B written per element. workspace:
+ *   b2v_image_normalize_f64_workspace_bytes, (imin, imax) in its first 16 bytes after the call.
+ * Empty shapes return B2V_OK untouched; negative sizes, null pointers and unknown surfaces are B2V_ERR_ARG. */
+#define B2V_TPMS_SCHWARZ_P 0
+#define B2V_TPMS_SCHWARZ_D 1
+#define B2V_TPMS_GYROID 2
+#define B2V_TPMS_NEOVIUS 3
+#define B2V_TPMS_IWP 4
+#define B2V_TPMS_P_W_HYBRID 5
+int b2v_tpms_f64(const double* tables, int64_t nz, int64_t ny, int64_t nx, int surface, double* out, void* stream);
+int64_t b2v_tpms_i16_workspace_bytes(int64_t nz, int64_t ny, int64_t nx);
+int b2v_tpms_i16(const double* tables, int64_t nz, int64_t ny, int64_t nx, int surface, double span, double min_f,
+                 int16_t fill, void* workspace, int16_t* out, void* stream);
+int64_t b2v_image_normalize_f64_workspace_bytes(int64_t n);
+int b2v_image_normalize_f64_i16(const double* in, int64_t n, double span, double min_f, int16_t fill, void* workspace,
+                                int16_t* out, void* stream);
+
 /* ---- binary morphology ---------------------------------------------------------------------------
  * b2v_binary_morphology: scipy.ndimage.binary_erosion(border_value=True) / binary_dilation(border_value=False)
  *   with the Euclidean footprint {d : |d|^2 <= radius^2}: skimage's disk(radius) on every z-slice alone

@@ -130,6 +130,11 @@ PROTOTYPES = {
     "b2v_jump_flooding": (cint, [vp, vp, i64, i64, i64, vp, i64, cint, vp, vp]),
     "b2v_voronoi_borders": (cint, [vp, i64, i64, i64, cint, vp, vp]),
     "b2v_image_normalize_f32_i16": (cint, [vp, i64, f32, f32, f32, f32, C.c_int16, vp, vp]),
+    "b2v_tpms_f64": (cint, [vp, i64, i64, i64, cint, vp, vp]),
+    "b2v_tpms_i16_workspace_bytes": (i64, [i64, i64, i64]),
+    "b2v_tpms_i16": (cint, [vp, i64, i64, i64, cint, dbl, dbl, C.c_int16, vp, vp, vp]),
+    "b2v_image_normalize_f64_workspace_bytes": (i64, [i64]),
+    "b2v_image_normalize_f64_i16": (cint, [vp, i64, dbl, dbl, C.c_int16, vp, vp, vp]),
     "b2v_binary_morphology_workspace_bytes": (i64, [i64, i64, i64, cint]),
     "b2v_binary_morphology": (cint, [vp, i64, i64, i64, u8, cint, cint, cint, u8, vp, vp, vp, vp]),
     "b2v_visibility_workspace_bytes": (i64, [i64, i64, cint]),
@@ -185,6 +190,8 @@ ZOOM_CONSTANT, ZOOM_MIRROR = 0, 1
 SEL_EQ, SEL_GT127 = 0, 1
 
 MORPH_ERODE, MORPH_DILATE = 0, 1
+
+TPMS_SURFACES = ("Schwarz P", "Schwarz D", "Gyroid", "Neovius", "iWP", "P_W_Hybrid")   # B2V_TPMS_* 0..5
 
 
 class Moments(C.Structure):

@@ -166,6 +166,14 @@ __device__ __forceinline__ T block_exscan(T x, T* s_w, T* total) {
   return base + inc - x;
 }
 
+// ---- imagedata_utils.image_normalize ---------------------------------------------------
+// One voxel of (image - imin) * scale + min_ in T's arithmetic (NumPy's, for a float32 or float64 image and
+// Python-scalar bounds), stored with the C cast: truncated into int32, low 16 bits kept (the x86 cast).
+template <typename T>
+__device__ __forceinline__ int16_t normalize_i16(T v, T imin, T scale, T min_f) {
+  return (int16_t)(int)((v - imin) * scale + min_f);
+}
+
 // ---- 3x3x3 structuring elements ---------------------------------------------------------
 // A uint8 element [odz][ody][odx] of at most 3 voxels on each axis, centred at (odz / 2, ody / 2, odx / 2), as
 // a 27-bit mask: bit (oz+1)*9 + (oy+1)*3 + (ox+1) stands for the offset (oz, oy, ox); bit 13 is the centre.

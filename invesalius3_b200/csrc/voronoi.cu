@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(kBx* kBy) k_voronoi_borders(const int32_t* __r
 
 // ---- image_normalize ----------------------------------------------------------------------------------------------
 // float32 throughout, as NumPy evaluates (image - imin) * (span / (imax - imin)) + min_ on a float32 image with
-// Python-scalar bounds; the int16 store truncates into int32 and keeps the low 16 bits (the x86 C cast).
+// Python-scalar bounds (normalize_i16; the float64 form is in porous.cu).
 __global__ void __launch_bounds__(256) k_image_normalize(const float* __restrict__ in, int64_t n, float imin, float imax,
                                                          float span, float min_f, int16_t fill,
                                                          int16_t* __restrict__ out) {
@@ -227,7 +227,7 @@ __global__ void __launch_bounds__(256) k_image_normalize(const float* __restrict
   const bool flat = imin == imax;
   const float scale = span / (imax - imin);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    out[i] = flat ? fill : (int16_t)(int)((in[i] - imin) * scale + min_f);
+    out[i] = flat ? fill : normalize_i16<float>(in[i], imin, scale, min_f);
 }
 
 struct Layout {
