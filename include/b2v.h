@@ -108,9 +108,8 @@ int64_t b2v_floodfill_workspace_bytes(int64_t dz, int64_t dy, int64_t dx, int64_
 /* Convergence engine of the flood-fill family: 1 (default) = every round inside ONE
  * persistent cooperative launch (rotating bitmaps of active tiles, grid-wide barrier per
  * round), 0 = one launch per round driven from the host. Same result either way.
- * Environment knobs read once per process (tuning only, results identical): B2V_FF_TILE=8
- * (small tiles), B2V_FF_TRIPS=n (sweep sets per tile visit), B2V_FF_GRID=n (blocks of the
- * persistent grid), B2V_FF_DEFER=n (surplus tiles a round may pass on). */
+ * Environment knob read once per process (tuning only, results identical): B2V_FF_GRID=n
+ * (blocks of the persistent grid). */
 void b2v_floodfill_set_engine(int persistent);
 int b2v_floodfill_threshold(const void* data, int dtype, int64_t dz, int64_t dy, int64_t dx,
                             const int64_t* seeds_host, int64_t nseeds, double t0, double t1, uint8_t fill,

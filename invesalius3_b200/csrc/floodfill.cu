@@ -27,20 +27,6 @@
 
 namespace cg = cooperative_groups;
 
-// Profiling counters of the flood engine (cycles per visit phase, tile visits) are compiled in
-// only with -DB2V_FF_STATS=1 (tools/flood_once.py builds read them through
-// b2v_floodfill_layout()[6]); the production kernels carry no clock reads or counter atomics.
-#ifndef B2V_FF_STATS
-#define B2V_FF_STATS 0
-#endif
-#if B2V_FF_STATS
-#define FF_CLK() clock64()
-#define FF_STAT(...) do { __VA_ARGS__; } while (0)
-#else
-#define FF_CLK() 0ll
-#define FF_STAT(...) do { } while (0)
-#endif
-
 namespace {
 
 constexpr int kTileWords = 4096;   // interior words of the largest tile (16 x 16 rows x 16 words = 131 072 voxels)
@@ -54,8 +40,6 @@ struct BitVol {
   int ntz, nty, ntw;   // tile grid
   int ltw, lty;        // log2(tw), log2(ty)
   uint32_t m_pw, m_pp; // ceil(2^24 / (tw+2)), ceil(2^24 / ((tw+2)(ty+2))): exact division for i < 2^12
-  int max_trips;       // local sweeps per visit before the tile re-queues itself
-  int defer;           // persistent engine: up to this many tiles beyond one per block wait a round
 };
 
 int pow2ceil(int64_t v, int cap) {
@@ -64,13 +48,11 @@ int pow2ceil(int64_t v, int cap) {
   return p;
 }
 
-// Tuning knobs (results identical either way), read from the environment ONCE per process.
+// Tuning knob (results identical either way), read from the environment ONCE per process:
+// B2V_FF_GRID=n caps the persistent grid at n blocks.
 struct FloodKnobs {
-  int edge = 16, trips = 1, defer = 1 << 30, grid = 0;
+  int grid = 0;
   FloodKnobs() {
-    if (const char* e = getenv("B2V_FF_TILE")) { if (atoi(e) == 8) edge = 8; }
-    if (const char* e = getenv("B2V_FF_TRIPS")) { int v = atoi(e); if (v > 0) trips = v; }
-    if (const char* e = getenv("B2V_FF_DEFER")) { int v = atoi(e); if (v >= 0) defer = v; }
     if (const char* e = getenv("B2V_FF_GRID")) { int v = atoi(e); if (v > 0) grid = v; }
   }
 };
@@ -84,12 +66,10 @@ BitVol make_bitvol(int64_t dz, int64_t dy, int64_t dx) {
   b.dz = dz; b.dy = dy; b.dx = dx;
   b.wx = (int)ceil_div64(dx, 32);
   // Tile edge (rows): 16 halves the number of rounds of a flood (one tile hop per round)
-  // against 8 for about twice the work per visit; B2V_FF_TILE=8 selects the small tile.
-  const int edge = knobs().edge;
-  const int words = edge == 16 ? kTileWords : 1024;
+  // against 8 for about twice the work per visit.
   b.tw = pow2ceil(b.wx, 16);
-  b.ty = pow2ceil(dy, edge);
-  b.tz = pow2ceil(dz, words / (b.tw * b.ty));
+  b.ty = pow2ceil(dy, 16);
+  b.tz = pow2ceil(dz, kTileWords / (b.tw * b.ty));
   // reached + passable tiles with halo must fit the 48 KB of default shared memory
   while (b.tz > 1 && (int64_t)(b.tz + 2) * (b.ty + 2) * (b.tw + 2) * 8 > 48 * 1024) b.tz >>= 1;
   b.ntz = (int)ceil_div64(dz, b.tz);
@@ -100,8 +80,6 @@ BitVol make_bitvol(int64_t dz, int64_t dy, int64_t dx) {
   const uint32_t pw = b.tw + 2, pp = (b.tw + 2) * (b.ty + 2);
   b.m_pw = ((1u << 24) + pw - 1) / pw;
   b.m_pp = ((1u << 24) + pp - 1) / pp;
-  b.max_trips = knobs().trips;   // default 1: one sweep set per visit, stragglers re-queue themselves
-  b.defer = knobs().defer;       // default: always cheaper than a second visit per block (any n <= 2 x blocks)
   return b;
 }
 
@@ -111,7 +89,7 @@ struct Workspace {
   uint8_t* active[2];
   int* flags;        // flags[r] != 0  <=>  some tile is active in round r
   int* lists;        // persistent engine: three rotating bitmaps of active tiles [3][ceil(ntiles / 32)]
-  int* ctl;          // [3] error, [4] tile visits, [5] visits that grew, [6] local iterations, [7] rounds
+  int* ctl;          // persistent engine: [3] error, [7] rounds, [16..18] peer exchange (k_ff_persistent)
   int64_t* seeds;    // device copy, 3 per seed
   int64_t bytes;
 };
@@ -293,7 +271,7 @@ __device__ __forceinline__ void sweep_col(uint32_t* sR, const uint32_t* sF, int 
 
 template <int LZ, int LY>
 __device__ __forceinline__ int ff_process_tile_sb6(const uint32_t* __restrict__ fg, uint32_t* reach, const BitVol& b,
-                                                   int tile, uint32_t* sR, int* s_faces, int* stats) {
+                                                   int tile, uint32_t* sR, int* s_faces) {
   constexpr int TZ = 1 << LZ, TY = 1 << LY, PW = 18, PY = TY + 2, NH = (TZ + 2) * PY * PW;
   constexpr int K = TZ * TY * 16 / kFloodThreads;          // words per thread
   constexpr int NL = (NH + kFloodThreads - 1) / kFloodThreads;
@@ -304,7 +282,6 @@ __device__ __forceinline__ int ff_process_tile_sb6(const uint32_t* __restrict__ 
   const int dz = (int)b.dz, dy = (int)b.dy;
   uint32_t* sF = sR + NH;
   if (tid == 0) *s_faces = 0;
-  const long long pc0 = FF_CLK();
   {
     uint32_t v[NL], f[NL];
 #pragma unroll
@@ -337,36 +314,30 @@ __device__ __forceinline__ int ff_process_tile_sb6(const uint32_t* __restrict__ 
     f[k] = sF[h];
     r0[k] = r[k] = sR[h];
   }
-  const long long pc1 = FF_CLK();
   const int iw = tid & 15;
-  int changed, iters = 0;
-  do {
-    int moved = 0;
-    // Each sweep is a serial chain in the registers of ONE thread per row / column (a few
-    // hundred threads busy, a few hundred cycles): far fewer instructions than a
-    // word-per-thread scan, and the block is latency-bound here, not width-bound.
-    if (tid < TZ * TY)        // x: row (z = tid >> LY, y = tid & (TY-1))
-      sweep_row_x(sR, sF, (((tid >> LY) + 1) * PY + ((tid & (TY - 1)) + 1)) * PW + 1);
-    __syncthreads();
-    if (tid < TZ * 16)        // y: column (z = tid >> 4, w = tid & 15), halo row y = -1 first
-      sweep_col<TY>(sR, sF, ((tid >> 4) + 1) * PY * PW + (tid & 15) + 1, PW);
-    __syncthreads();
-    if (tid < TY * 16)        // z: column (y = tid >> 4, w = tid & 15), halo plane z = -1 first
-      sweep_col<TZ>(sR, sF, ((tid >> 4) + 1) * PW + (tid & 15) + 1, PY * PW);
-    __syncthreads();
+  // Each sweep is a serial chain in the registers of ONE thread per row / column (a few
+  // hundred threads busy, a few hundred cycles): far fewer instructions than a
+  // word-per-thread scan, and the block is latency-bound here, not width-bound.
+  if (tid < TZ * TY)        // x: row (z = tid >> LY, y = tid & (TY-1))
+    sweep_row_x(sR, sF, (((tid >> LY) + 1) * PY + ((tid & (TY - 1)) + 1)) * PW + 1);
+  __syncthreads();
+  if (tid < TZ * 16)        // y: column (z = tid >> 4, w = tid & 15), halo row y = -1 first
+    sweep_col<TY>(sR, sF, ((tid >> 4) + 1) * PY * PW + (tid & 15) + 1, PW);
+  __syncthreads();
+  if (tid < TY * 16)        // z: column (y = tid >> 4, w = tid & 15), halo plane z = -1 first
+    sweep_col<TZ>(sR, sF, ((tid >> 4) + 1) * PW + (tid & 15) + 1, PY * PW);
+  __syncthreads();
+  int moved = 0;
 #pragma unroll
-    for (int k = 0; k < K; ++k) {
-      const int i = tid + k * kFloodThreads;
-      const int h = (((i >> (4 + LY)) + 1) * PY + (((i >> 4) & (TY - 1)) + 1)) * PW + iw + 1;
-      const uint32_t v = sR[h];
-      moved |= v != r[k];
-      r[k] = v;
-    }
-    changed = __syncthreads_or(moved);
-    ++iters;
-  } while (changed && iters < b.max_trips);
-  const bool unfinished = changed != 0;
-  const long long pc2 = FF_CLK();
+  for (int k = 0; k < K; ++k) {
+    const int i = tid + k * kFloodThreads;
+    const int h = (((i >> (4 + LY)) + 1) * PY + (((i >> 4) & (TY - 1)) + 1)) * PW + iw + 1;
+    const uint32_t v = sR[h];
+    moved |= v != r[k];
+    r[k] = v;
+  }
+  // one sweep set per visit: a tile that changed may not be settled yet and re-queues itself
+  const bool unfinished = __syncthreads_or(moved) != 0;
   int grew = 0;
 #pragma unroll
   for (int k = 0; k < K; ++k)
@@ -376,16 +347,6 @@ __device__ __forceinline__ int ff_process_tile_sb6(const uint32_t* __restrict__ 
       grew = 1;
     }
   grew = __syncthreads_or(grew);
-  const long long pc3 = FF_CLK();
-  FF_STAT(if (tid == 0) {
-    atomicAdd(&stats[11], (int)((pc1 - pc0) >> 4));
-    atomicAdd(&stats[12], (int)((pc2 - pc1) >> 4));
-    atomicAdd(&stats[13], (int)((pc3 - pc2) >> 4));
-    atomicAdd(&stats[4], 1);
-    if (grew) atomicAdd(&stats[5], 1);
-    atomicAdd(&stats[6], iters);
-  });
-  (void)pc0; (void)pc1; (void)pc2; (void)pc3; (void)stats;
   // which of the six face neighbours can gain a bit from this tile's interior? One face word
   // per thread: passable-but-unreached bits of the halo word against the reached bits of the
   // interior word next to it (same bit across y / z, the adjacent bit across a word boundary).
@@ -415,16 +376,14 @@ __device__ __forceinline__ int ff_process_tile_sb6(const uint32_t* __restrict__ 
   }
   if (unfinished && tid == 0) atomicOr(s_faces, 1 << 13);   // (0,0,0): re-queue this tile itself
   __syncthreads();
-  FF_STAT(if (tid == 0) atomicAdd(&stats[14], (int)((clock64() - pc3) >> 4)));
   return *s_faces;
 }
 
 template <uint32_t SBC>
 __device__ __forceinline__ int ff_process_tile(const uint32_t* __restrict__ fg, uint32_t* reach, const BitVol& b,
-                                               uint32_t sb_rt, int tile, uint32_t* sR, int* s_faces, int* stats) {
+                                               uint32_t sb_rt, int tile, uint32_t* sR, int* s_faces) {
   if constexpr (SBC == kSB6) {
-    if (b.tw == 16 && b.ty == 16 && b.tz == 16) return ff_process_tile_sb6<4, 4>(fg, reach, b, tile, sR, s_faces, stats);
-    if (b.tw == 16 && b.ty == 8 && b.tz == 8) return ff_process_tile_sb6<3, 3>(fg, reach, b, tile, sR, s_faces, stats);
+    if (b.tw == 16 && b.ty == 16 && b.tz == 16) return ff_process_tile_sb6<4, 4>(fg, reach, b, tile, sR, s_faces);
   }
   const uint32_t sb = SBC ? SBC : sb_rt;
   // the x sweep needs both x offsets; a one-sided x offset is left to the generic hop
@@ -436,7 +395,6 @@ __device__ __forceinline__ int ff_process_tile(const uint32_t* __restrict__ fg, 
   const int64_t z0 = (int64_t)tzi * tz, y0 = (int64_t)tyi * ty;
   const int w0 = twi * tw;
   if (tid == 0) *s_faces = 0;
-  const long long pc0 = FF_CLK();
   // halo load (zero outside the volume); the passable bits ride along (halo words are
   // never written)
   const int nh = (tz + 2) * py * pw;
@@ -495,110 +453,103 @@ __device__ __forceinline__ int ff_process_tile(const uint32_t* __restrict__ fg, 
       fgr[k] = sF[hidx[k]];
     }
 
-  const long long pc1 = FF_CLK();
   const bool xfill = ((sb >> 12) & 1u) && ((sb >> 14) & 1u);  // (0,0,-1) and (0,0,+1)
   // axis-aligned offsets present in the structuring element (flood moves p -> p + off)
   const bool yfwd = (sb >> 16) & 1u, ybwd = (sb >> 10) & 1u;   // (0,+1,0), (0,-1,0)
   const bool zfwd = (sb >> 22) & 1u, zbwd = (sb >> 4) & 1u;    // (+1,0,0), (-1,0,0)
-  int changed;
-  int iters = 0;
-  do {
-    changed = 0;
-    // ---- directional sweeps: each carries reached bits across the whole tile along one
-    // axis in O(1) dependent steps (a Jacobi step moves them by one row / one word only)
-    if (xfill) {
-      // Along x a row is a chain of words. Per word: fill the runs that already hold a
-      // reached bit; g = "the fill reaches the word's last bit" (carry generate), p = "the
-      // word is all passable" (carry propagate). The carries into every word of the row
-      // are then one integer addition (carry-lookahead): (a + b + c0) ^ a ^ b with
-      // a = g | p, b = g. Same towards lower x on the bit-reversed masks.
-      const int lane = tid & 31;
-      const int grp = lane >> b.ltw;                   // tw is a power of two <= 16
-      const uint32_t gmask = (tw == 32) ? 0xffffffffu : ((1u << tw) - 1u);
-      for (int i0 = 0; i0 < nint || i0 == 0; i0 += kFloodThreads) {
-        const int i = i0 + tid;
-        const bool live = i < nint;
-        const int row = live ? i >> b.ltw : 0, w = live ? i & (tw - 1) : 0;
-        const int base = (((row >> b.lty) + 1) * py + ((row & (ty - 1)) + 1)) * pw + 1;
-        uint32_t f = 0, cur = 0, filled = 0;
-        if (live) {
-          f = sF[base + w];
-          cur = sR[base + w];
-          filled = (f && cur) ? run_fill(cur & f, f) : 0u;
-        }
-        const bool pfull = live && f == 0xffffffffu;
-        const uint32_t gu = (__ballot_sync(0xffffffffu, filled >> 31) >> (grp * tw)) & gmask;
-        const uint32_t gd = (__ballot_sync(0xffffffffu, filled & 1u) >> (grp * tw)) & gmask;
-        const uint32_t pm = (__ballot_sync(0xffffffffu, pfull) >> (grp * tw)) & gmask;
-        if (live) {
-          // up: carry into word k = bit k of the carry vector; the left halo word feeds bit 0
-          const uint32_t c0 = sR[base - 1] >> 31;
-          const uint32_t au = gu | pm, bu = gu;
-          const uint32_t cu = ((au + bu + c0) ^ au ^ bu);
-          // down: reverse the word order so that the same adder runs towards lower x
-          const uint32_t gdr = __brev(gd) >> (32 - tw), pmr = __brev(pm) >> (32 - tw);
-          const uint32_t c1 = sR[base + tw] & 1u;
-          const uint32_t ad = gdr | pmr, bd = gdr;
-          const uint32_t cd = ((ad + bd + c1) ^ ad ^ bd);
-          const uint32_t cin_lo = (cu >> w) & 1u;                 // enters at bit 0
-          const uint32_t cin_hi = (cd >> (tw - 1 - w)) & 1u;      // enters at bit 31
-          const uint32_t seed = (cur | cin_lo | (cin_hi << 31)) & f;
-          const uint32_t v = seed ? run_fill(seed, f) : 0u;
-          if (v != cur) { sR[base + w] = v; changed = 1; }
-        }
+  int changed = 0;
+  // ---- directional sweeps: each carries reached bits across the whole tile along one
+  // axis in O(1) dependent steps (a Jacobi step moves them by one row / one word only)
+  if (xfill) {
+    // Along x a row is a chain of words. Per word: fill the runs that already hold a
+    // reached bit; g = "the fill reaches the word's last bit" (carry generate), p = "the
+    // word is all passable" (carry propagate). The carries into every word of the row
+    // are then one integer addition (carry-lookahead): (a + b + c0) ^ a ^ b with
+    // a = g | p, b = g. Same towards lower x on the bit-reversed masks.
+    const int lane = tid & 31;
+    const int grp = lane >> b.ltw;                   // tw is a power of two <= 16
+    const uint32_t gmask = (tw == 32) ? 0xffffffffu : ((1u << tw) - 1u);
+    for (int i0 = 0; i0 < nint || i0 == 0; i0 += kFloodThreads) {
+      const int i = i0 + tid;
+      const bool live = i < nint;
+      const int row = live ? i >> b.ltw : 0, w = live ? i & (tw - 1) : 0;
+      const int base = (((row >> b.lty) + 1) * py + ((row & (ty - 1)) + 1)) * pw + 1;
+      uint32_t f = 0, cur = 0, filled = 0;
+      if (live) {
+        f = sF[base + w];
+        cur = sR[base + w];
+        filled = (f && cur) ? run_fill(cur & f, f) : 0u;
       }
-      __syncthreads();
-    }
-    if (yfwd || ybwd) {
-      // one thread per (z, word) column
-      for (int c = tid; c < tz * tw; c += kFloodThreads) {
-        const int base = (((c >> b.ltw) + 1) * py) * pw + ((c & (tw - 1)) + 1);  // halo row hy = 0
-        changed |= sweep_column(sR, sF, base, pw, ty, yfwd, ybwd);
+      const bool pfull = live && f == 0xffffffffu;
+      const uint32_t gu = (__ballot_sync(0xffffffffu, filled >> 31) >> (grp * tw)) & gmask;
+      const uint32_t gd = (__ballot_sync(0xffffffffu, filled & 1u) >> (grp * tw)) & gmask;
+      const uint32_t pm = (__ballot_sync(0xffffffffu, pfull) >> (grp * tw)) & gmask;
+      if (live) {
+        // up: carry into word k = bit k of the carry vector; the left halo word feeds bit 0
+        const uint32_t c0 = sR[base - 1] >> 31;
+        const uint32_t au = gu | pm, bu = gu;
+        const uint32_t cu = ((au + bu + c0) ^ au ^ bu);
+        // down: reverse the word order so that the same adder runs towards lower x
+        const uint32_t gdr = __brev(gd) >> (32 - tw), pmr = __brev(pm) >> (32 - tw);
+        const uint32_t c1 = sR[base + tw] & 1u;
+        const uint32_t ad = gdr | pmr, bd = gdr;
+        const uint32_t cd = ((ad + bd + c1) ^ ad ^ bd);
+        const uint32_t cin_lo = (cu >> w) & 1u;                 // enters at bit 0
+        const uint32_t cin_hi = (cd >> (tw - 1 - w)) & 1u;      // enters at bit 31
+        const uint32_t seed = (cur | cin_lo | (cin_hi << 31)) & f;
+        const uint32_t v = seed ? run_fill(seed, f) : 0u;
+        if (v != cur) { sR[base + w] = v; changed = 1; }
       }
-      __syncthreads();
     }
-    if (zfwd || zbwd) {
-      // one thread per (y, word) column
-      for (int c = tid; c < ty * tw; c += kFloodThreads) {
-        const int base = ((c >> b.ltw) + 1) * pw + ((c & (tw - 1)) + 1);         // halo plane hz = 0
-        changed |= sweep_column(sR, sF, base, py * pw, tz, zfwd, zbwd);
-      }
-      __syncthreads();
+    __syncthreads();
+  }
+  if (yfwd || ybwd) {
+    // one thread per (z, word) column
+    for (int c = tid; c < tz * tw; c += kFloodThreads) {
+      const int base = (((c >> b.ltw) + 1) * py) * pw + ((c & (tw - 1)) + 1);  // halo row hy = 0
+      changed |= sweep_column(sR, sF, base, pw, ty, yfwd, ybwd);
     }
-    // ---- generic step: every offset of the structuring element, one hop
-    if (!axis_only)
+    __syncthreads();
+  }
+  if (zfwd || zbwd) {
+    // one thread per (y, word) column
+    for (int c = tid; c < ty * tw; c += kFloodThreads) {
+      const int base = ((c >> b.ltw) + 1) * pw + ((c & (tw - 1)) + 1);         // halo plane hz = 0
+      changed |= sweep_column(sR, sF, base, py * pw, tz, zfwd, zbwd);
+    }
+    __syncthreads();
+  }
+  // ---- generic step: every offset of the structuring element, one hop
+  if (!axis_only)
 #pragma unroll
-    for (int k = 0; k < kOwn; ++k) {
-      if (hidx[k] < 0 || fgr[k] == 0) continue;
-      uint32_t cur = sR[hidx[k]];
-      if (cur == fgr[k]) continue;  // saturated
-      uint32_t acc = cur;
+  for (int k = 0; k < kOwn; ++k) {
+    if (hidx[k] < 0 || fgr[k] == 0) continue;
+    uint32_t cur = sR[hidx[k]];
+    if (cur == fgr[k]) continue;  // saturated
+    uint32_t acc = cur;
 #pragma unroll
-      for (int oz = -1; oz <= 1; ++oz) {
+    for (int oz = -1; oz <= 1; ++oz) {
 #pragma unroll
-        for (int oy = -1; oy <= 1; ++oy) {
-          uint32_t xm = (sb >> ((oz + 1) * 9 + (oy + 1) * 3)) & 7u;
-          if (xm == 0) continue;
-          int src = hidx[k] - (oz * py + oy) * pw;  // row (z - oz, y - oy)
-          uint32_t c = sR[src];
-          if (xm & 2u) acc |= c;
-          if (xm & 4u) acc |= (c << 1) | (sR[src - 1] >> 31);  // ox = +1
-          if (xm & 1u) acc |= (c >> 1) | (sR[src + 1] << 31);  // ox = -1
-        }
-      }
-      acc &= fgr[k];
-      if (xfill && acc) acc = run_fill(acc, fgr[k]);
-      if (acc != cur) {
-        sR[hidx[k]] = acc;
-        changed = 1;
+      for (int oy = -1; oy <= 1; ++oy) {
+        uint32_t xm = (sb >> ((oz + 1) * 9 + (oy + 1) * 3)) & 7u;
+        if (xm == 0) continue;
+        int src = hidx[k] - (oz * py + oy) * pw;  // row (z - oz, y - oy)
+        uint32_t c = sR[src];
+        if (xm & 2u) acc |= c;
+        if (xm & 4u) acc |= (c << 1) | (sR[src - 1] >> 31);  // ox = +1
+        if (xm & 1u) acc |= (c >> 1) | (sR[src + 1] << 31);  // ox = -1
       }
     }
-    changed = __syncthreads_or(changed);
-    ++iters;
-  } while (changed && iters < b.max_trips);
-  const bool unfinished = changed != 0;   // trip cap hit: this tile must be visited again
+    acc &= fgr[k];
+    if (xfill && acc) acc = run_fill(acc, fgr[k]);
+    if (acc != cur) {
+      sR[hidx[k]] = acc;
+      changed = 1;
+    }
+  }
+  // one sweep set per visit: a tile that changed may not be settled yet and re-queues itself
+  const bool unfinished = __syncthreads_or(changed) != 0;
 
-  const long long pc2 = FF_CLK();
   // write back what grew
   int grew = 0;
 #pragma unroll
@@ -619,16 +570,6 @@ __device__ __forceinline__ int ff_process_tile(const uint32_t* __restrict__ fg, 
   int nbmask = 0;
   // (checked even without growth: a lone seed on a tile face must still wake its neighbour)
   grew = __syncthreads_or(grew);
-  const long long pc3 = FF_CLK();
-  FF_STAT(if (tid == 0) {   // stats[4] tile visits, [5] visits that grew, [6] local iterations
-    atomicAdd(&stats[11], (int)((pc1 - pc0) >> 4));   // cycles/16: halo load
-    atomicAdd(&stats[12], (int)((pc2 - pc1) >> 4));   //            local convergence
-    atomicAdd(&stats[13], (int)((pc3 - pc2) >> 4));   //            write back
-    atomicAdd(&stats[4], 1);
-    if (grew) atomicAdd(&stats[5], 1);
-    atomicAdd(&stats[6], iters);
-  });
-  (void)pc0; (void)pc1; (void)pc2; (void)pc3; (void)stats;
   {
     const int hzmax = tz + 1, hymax = ty + 1, hwmax = tw + 1;
     for (int i = tid; i < nh; i += kFloodThreads) {
@@ -664,14 +605,13 @@ __device__ __forceinline__ int ff_process_tile(const uint32_t* __restrict__ fg, 
   if (unfinished && tid == 0) nbmask |= 1 << 13;   // (0,0,0): re-queue this tile itself
   if (nbmask) atomicOr(s_faces, nbmask);
   __syncthreads();
-  FF_STAT(if (tid == 0) atomicAdd(&stats[14], (int)((clock64() - pc3) >> 4)));   // neighbour gain test
   return *s_faces;
 }
 
 template <uint32_t SBC>
 __global__ void __launch_bounds__(kFloodThreads)
     k_ff_round(const uint32_t* __restrict__ fg, uint32_t* reach, BitVol b, uint32_t sb, uint8_t* active_cur,
-               uint8_t* active_next, int* flags, int round, int* stats) {
+               uint8_t* active_next, int* flags, int round) {
   if (flags[round] == 0) return;
   const int tile = blockIdx.x;
   // consistent decision for the whole block before thread 0 clears the entry
@@ -681,7 +621,7 @@ __global__ void __launch_bounds__(kFloodThreads)
   const int tid = threadIdx.x;
   if (tid == 0) active_cur[tile] = 0;  // this buffer becomes `next` of the following round
   const int twi = tile % b.ntw, tyi = (tile / b.ntw) % b.nty, tzi = tile / (b.ntw * b.nty);
-  const int nbmask = ff_process_tile<SBC>(fg, reach, b, sb, tile, sR, &s_faces, stats);
+  const int nbmask = ff_process_tile<SBC>(fg, reach, b, sb, tile, sR, &s_faces);
   if (nbmask == 0) return;
   __threadfence();
   // activate the neighbour tiles that can gain from this one
@@ -783,7 +723,7 @@ __device__ __forceinline__ int ff_select_tiles(const uint32_t* bm, int nbw, int 
   return base;
 }
 
-// CANON = log2 of the tile edge (3, 4): 6-connected flood on that canonical tile only
+// CANON = 4: 6-connected flood on the canonical 16 x 16 rows x 16 words tile only
 // (ff_process_tile_sb6, no generic path); 0 = any tile, any element.
 // (Two co-resident blocks per SM at 32 registers were measured slower: the barrier doubles
 // and the visits of the two blocks contend.)
@@ -804,10 +744,8 @@ __global__ void __launch_bounds__(kFloodThreads)
   __shared__ int s_mine[kMaxMine];
   const int tid = threadIdx.x;
   int r = 0, outer = 0;
-  long long c_proc = 0, c_sync = 0, c_all0 = FF_CLK();
   for (;;) {
   for (;; ++r) {
-    const long long c0 = FF_CLK();
     const int cur = r % 3, nxt = (r + 1) % 3, old = (r + 2) % 3;
     const int n = ff_select_tiles(bm + (size_t)cur * nbw, nbw, blockIdx.x, gridDim.x, s_mine, s_wsum);
     if (n == 0) break;
@@ -816,9 +754,9 @@ __global__ void __launch_bounds__(kFloodThreads)
     for (int i = blockIdx.x * kFloodThreads + tid; i < nbw; i += gridDim.x * kFloodThreads) bm[(size_t)old * nbw + i] = 0;
     int nmine = n > (int)blockIdx.x ? (n - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     int keep = -1;
-    if (b.defer && nmine == 2 && n - (int)gridDim.x <= b.defer) {
+    if (nmine == 2) {
       // a few tiles more than blocks: pass them on to the next round instead of making every
-      // block wait for a second visit
+      // block wait for a second visit (always the cheaper of the two while n <= 2 x blocks)
       // (alternating which of the two waits, so that no tile waits twice in a row)
       const int t = s_mine[(r & 1) ? 0 : 1];
       keep = s_mine[(r & 1) ? 1 : 0];
@@ -828,8 +766,8 @@ __global__ void __launch_bounds__(kFloodThreads)
     for (int k = 0; k < nmine; ++k) {
       const int tile = keep >= 0 ? keep : s_mine[k];
       int nbmask;
-      if constexpr (CANON != 0) nbmask = ff_process_tile_sb6<CANON, CANON>(fg, reach, b, tile, sR, &s_faces, ctl);
-      else nbmask = ff_process_tile<SBC>(fg, reach, b, sb, tile, sR, &s_faces, ctl);
+      if constexpr (CANON != 0) nbmask = ff_process_tile_sb6<CANON, CANON>(fg, reach, b, tile, sR, &s_faces);
+      else nbmask = ff_process_tile<SBC>(fg, reach, b, sb, tile, sR, &s_faces);
       if (tid < 27 && ((nbmask >> tid) & 1)) {
         const int twi = tile % b.ntw, tyi = (tile / b.ntw) % b.nty, tzi = tile / (b.ntw * b.nty);
         int oz = tid / 9 - 1, oy = (tid / 3) % 3 - 1, ow = tid % 3 - 1;
@@ -841,11 +779,7 @@ __global__ void __launch_bounds__(kFloodThreads)
       }
       __syncthreads();   // s_faces / shared tile are reused by the next tile of this block
     }
-    const long long c1 = FF_CLK();
     grid.sync();   // orders every thread's writes (reach words, next bitmap) before the next round's reads
-    const long long c2 = FF_CLK();
-    c_proc += c1 - c0;
-    c_sync += c2 - c1;
   }
   if constexpr (!PEER) {
     break;
@@ -936,10 +870,6 @@ __global__ void __launch_bounds__(kFloodThreads)
   if (blockIdx.x == 0 && tid == 0) {
     ctl[7] = r;
     ctl[18] = outer;
-    FF_STAT(ctl[8] = (int)(c_proc >> 4);    // block 0: cycles/16 spent on its tiles ...
-            ctl[9] = (int)(c_sync >> 4);    // ... and in fence + grid barrier (incl. waiting for slower blocks)
-            ctl[10] = (int)((clock64() - c_all0) >> 4));
-    (void)c_proc; (void)c_sync; (void)c_all0;
   }
 }
 
@@ -1004,7 +934,7 @@ int run_rounds(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_t s,
     for (int k = 0; k < batch; ++k, ++r) {
 #define B2V_FF_ROUND(SBC)                                                                                     \
   k_ff_round<SBC><<<ntiles, kFloodThreads, smem, s>>>(w.fg, w.reach, b, sb, w.active[r & 1], w.active[(r + 1) & 1], \
-                                                      w.flags, r, w.ctl)
+                                                      w.flags, r)
       if (sb == kSB6) B2V_FF_ROUND(kSB6);
       else if (sb == kSB26) B2V_FF_ROUND(kSB26);
       else if (sb == kSB18) B2V_FF_ROUND(kSB18);
@@ -1054,14 +984,12 @@ int run_persistent(const BitVol& b, const Workspace& w, uint32_t sb, cudaStream_
   int rc;
   const int nbw = (int)((ntiles + 31) / 32);
   uint32_t* bm = (uint32_t*)w.lists;   // three rotating tile bitmaps [3][nbw]
-  const int canon = (sb == kSB6 && b.tw == 16 && b.ty == b.tz) ? (b.ty == 16 ? 4 : b.ty == 8 ? 3 : 0) : 0;
-  void* kern = peer ? (canon == 4 ? (void*)k_ff_persistent<kSB6, 4, true>
-                      : canon == 3 ? (void*)k_ff_persistent<kSB6, 3, true>
+  const bool canon = sb == kSB6 && b.tw == 16 && b.ty == 16 && b.tz == 16;
+  void* kern = peer ? (canon ? (void*)k_ff_persistent<kSB6, 4, true>
                       : sb == kSB6 ? (void*)k_ff_persistent<kSB6, 0, true>
                       : sb == kSB26 ? (void*)k_ff_persistent<kSB26, 0, true>
                       : sb == kSB18 ? (void*)k_ff_persistent<kSB18, 0, true> : (void*)k_ff_persistent<0u, 0, true>)
-                    : (canon == 4 ? (void*)k_ff_persistent<kSB6, 4, false>
-                      : canon == 3 ? (void*)k_ff_persistent<kSB6, 3, false>
+                    : (canon ? (void*)k_ff_persistent<kSB6, 4, false>
                       : sb == kSB6 ? (void*)k_ff_persistent<kSB6, 0, false>
                       : sb == kSB26 ? (void*)k_ff_persistent<kSB26, 0, false>
                       : sb == kSB18 ? (void*)k_ff_persistent<kSB18, 0, false> : (void*)k_ff_persistent<0u, 0, false>);
@@ -1312,7 +1240,7 @@ extern "C" int b2v_floodfill_layout(int64_t dz, int64_t dy, int64_t dx, int64_t 
   layout_out[3] = (int64_t)b.dy * b.wx * 4;  // bytes per z-plane of a bit volume
   layout_out[4] = (int64_t)b.ntz * b.nty * b.ntw;
   layout_out[5] = kMaxRounds;
-  layout_out[6] = (int64_t)((char*)w.ctl - (char*)nullptr);  // int32 ctl[]: [4] tile visits, [5] grew, [6] iterations
+  layout_out[6] = (int64_t)((char*)w.ctl - (char*)nullptr);  // int32 ctl[]: [7] rounds of the persistent kernel
   return B2V_OK;
 }
 

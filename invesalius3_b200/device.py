@@ -364,7 +364,8 @@ def floodfill_threshold(data: torch.Tensor, seeds, t0, t1, fill: int, strct, out
     """Region grow from `seeds` ((x, y, z) triples) through voxels with t0 <= data <= t1 that
     are not already `fill` in `out`; reached voxels get out = fill (floodfill.rs:96-166).
     Returns the number of flood rounds. Synchronises the stream. `stats` (optional dict)
-    receives tile_visits / visits_that_grew / local_iterations of the flood."""
+    receives `tiles`, the tile count of the flood, and `rounds`, the persistent kernel's own
+    round count (0 when the host-driven rounds ran)."""
     _dense(data, "data"); _dense(out, "out")
     if out.dtype != torch.uint8 or out.shape != data.shape or data.dim() != 3:
         raise TypeError("floodfill_threshold: out must be uint8 with data's 3-D shape")
@@ -382,11 +383,7 @@ def floodfill_threshold(data: torch.Tensor, seeds, t0, t1, fill: int, strct, out
         lay = (C.c_int64 * 8)()
         _lib.call("b2v_floodfill_layout", dz, dy, dx, max(len(s), 1), lay)
         ctl = ws[lay[6]: lay[6] + 64].view(torch.int32).cpu().tolist()
-        stats.update(tile_visits=ctl[4], visits_that_grew=ctl[5], local_iterations=ctl[6],
-                     tiles=int(lay[4]), rounds=ctl[7], block0_cycles_processing=ctl[8] * 16,
-                     block0_cycles_barrier=ctl[9] * 16, block0_cycles_total=ctl[10] * 16,
-                     cycles_halo_load=ctl[11] * 16, cycles_converge=ctl[12] * 16, cycles_writeback=ctl[13] * 16,
-                     cycles_gain_test=ctl[14] * 16)
+        stats.update(tiles=int(lay[4]), rounds=ctl[7])
     return rounds.value
 
 

@@ -1,6 +1,6 @@
-"""Flood-fill cases under the tuning knobs B2V_FF_TILE, B2V_FF_GRID, B2V_FF_TRIPS and B2V_FF_DEFER.
+"""Flood-fill cases under the tuning knob B2V_FF_GRID.
 
-The knobs are read once per process (`FloodKnobs` in csrc/floodfill.cu), so every setting floods
+The knob is read once per process (`FloodKnobs` in csrc/floodfill.cu), so every setting floods
 in a process of its own:
 
     python tests/ff_knob_child.py SETTING OUTDIR
@@ -10,7 +10,6 @@ and OUTDIR/results.json (returned round count and `stats` per flood). The cases 
 tests/test_gpu_floodfill_paths.py rebuilds the same inputs for the serial checker."""
 from __future__ import annotations
 
-import functools
 import json
 import sys
 import zlib
@@ -36,35 +35,24 @@ ELEMENTS = {"6": generate_binary_structure(3, 1), "18": generate_binary_structur
             "26": generate_binary_structure(3, 3), "asym": ASYM}
 SYMMETRIC = ("6", "18", "26")
 
-CANON = (37, 45, 1100)      # canonical tiles at either edge: 16 x 16 rows x 16 words, or 8 x 8 x 16
-NONCANON = (60, 90, 250)    # 8-word rows: generic tiles (32 x 16 x 8 words, or 16 x 8 x 8)
-BIG = (512, 512, 512)       # 4096 canonical tiles at edge 8: the block-wide tile ranking
+CANON = (37, 45, 1100)      # canonical tiles: 16 x 16 rows x 16 words
+NONCANON = (60, 90, 250)    # 8-word rows: generic tiles (32 x 16 x 8 words)
 
 # name -> (environment, {case shape name: (z, y, x)}). "own": a few hundred tiles, one seed in each,
 # so that a block owns up to MAX_MINE tiles in the first round; "fallback": more tiles than
 # grid * MAX_MINE, which the persistent engine hands to the host-driven rounds.
 SETTINGS = {
-    "tile8": ({"B2V_FF_TILE": "8"}, {"canon": CANON, "noncanon": NONCANON, "big": BIG}),
     "grid1": ({"B2V_FF_GRID": "1"}, {"canon": CANON, "noncanon": NONCANON, "own": (4, 4096, 64),
                                       "fallback": (4, 4112, 64)}),
     "grid3": ({"B2V_FF_GRID": "3"}, {"canon": CANON, "noncanon": NONCANON, "own": (4, 4800, 64),
                                       "fallback": (4, 12304, 64)}),
-    "trips3": ({"B2V_FF_TRIPS": "3"}, {"canon": CANON, "noncanon": NONCANON}),
-    "defer0": ({"B2V_FF_DEFER": "0"}, {"canon": CANON, "noncanon": NONCANON}),
-    "tile8_grid2": ({"B2V_FF_TILE": "8", "B2V_FF_GRID": "2"}, {"canon": CANON, "noncanon": NONCANON,
-                                                               "own": (4, 4096, 64), "fallback": (4, 4104, 64)}),
 }
 
 
-def tile_edge(setting: str) -> int:
-    return 8 if SETTINGS[setting][0].get("B2V_FF_TILE") == "8" else 16
-
-
-def tile_shape(shape, edge: int = 16):
+def tile_shape(shape):
     """make_bitvol() restated: tile dims (planes, rows, words) and the tile grid."""
     dz, dy, dx = shape
     wx = -(-dx // 32)
-    words = 4096 if edge == 16 else 1024
 
     def pow2ceil(v, cap):
         p = 1
@@ -73,41 +61,25 @@ def tile_shape(shape, edge: int = 16):
         return p
 
     tw = pow2ceil(wx, 16)
-    ty = pow2ceil(dy, edge)
-    tz = pow2ceil(dz, words // (tw * ty))
+    ty = pow2ceil(dy, 16)
+    tz = pow2ceil(dz, 4096 // (tw * ty))
     while tz > 1 and (tz + 2) * (ty + 2) * (tw + 2) * 8 > 48 * 1024:
         tz >>= 1
     return (tz, ty, tw), (-(-dz // tz), -(-dy // ty), -(-wx // tw))
 
 
-def tile_count(shape, edge: int = 16) -> int:
-    _, (nz, ny, nw) = tile_shape(shape, edge)
+def tile_count(shape) -> int:
+    _, (nz, ny, nw) = tile_shape(shape)
     return nz * ny * nw
-
-
-@functools.lru_cache(maxsize=1)
-def _phantom(shape):
-    from invesalius3_b200 import phantom
-    return phantom.ct(shape, seed=2)
-
-
-def elements_for(sname: str):
-    return ("6", "26") if sname == "big" else tuple(ELEMENTS)
 
 
 def cases(setting: str):
     """(case name, shape name, element name) of every flood of the setting."""
-    return [(f"{sname}-{ename}", sname, ename) for sname in SETTINGS[setting][1] for ename in elements_for(sname)]
+    return [(f"{sname}-{ename}", sname, ename) for sname in SETTINGS[setting][1] for ename in ELEMENTS]
 
 
 def case_inputs(setting: str, sname: str, ename: str) -> dict:
     shape = SETTINGS[setting][1][sname]
-    if sname == "big":
-        from invesalius3_b200 import phantom
-        data = _phantom(shape)
-        seeds = [phantom.first_seed_in_range(data, shape[0] // 2, 226, 3071)]
-        return dict(data=data, seeds=seeds, t0=226, t1=3071, fill=254, strct=ELEMENTS[ename],
-                    out0=np.zeros(shape, np.uint8))
     key = zlib.crc32(f"{setting}/{sname}/{ename}".encode())
     rng = np.random.default_rng(key)
     f = ndimage.gaussian_filter(rng.normal(size=shape), 2.0)
@@ -118,7 +90,7 @@ def case_inputs(setting: str, sname: str, ename: str) -> dict:
     inr = (data >= t0) & (data <= t1)
     seeds = []
     if sname in ("own", "fallback"):
-        ty = tile_shape(shape, tile_edge(setting))[0][1]
+        ty = tile_shape(shape)[0][1]
         for y0 in range(0, shape[1], ty):          # the tiles are bands of ty rows: one seed in each
             band = inr[:, y0:y0 + ty]
             idx = np.flatnonzero(band)

@@ -298,12 +298,12 @@ def test_floodfill_wide_rows_many_x_tiles(rs, orc):
         assert (want == 200).sum() > 1000
 
 
-@pytest.mark.parametrize("shape", [(37, 45, 1100), (16, 16, 544), (33, 17, 2048)])
+@pytest.mark.parametrize("shape", [(37, 45, 1100), (16, 16, 544), (33, 17, 2048), (8, 8, 1100)])
 def test_floodfill_canonical_tiles_across_x(rs, orc, shape):
     """The 6-connected fast path on 16 x 16 x 16-word tiles with several tiles along x (rows
     wider than 512 voxels), partial tiles on every side: the run fill has to cross word and
-    tile boundaries through the halo words. Also in place. (The small tiles of B2V_FF_TILE=8
-    need a process of their own: test_gpu_floodfill_paths.py.)"""
+    tile boundaries through the halo words. Also in place. (8 x 8 x 1100 has 8 x 8-row tiles,
+    which the generic 6-connected tile processor takes.)"""
     rng = np.random.default_rng(31)
     # long thin structures along x so that the flood travels through many x tiles
     data = (ndimage.gaussian_filter(rng.normal(size=shape), (1.5, 1.5, 12)) > 0.0).astype(np.int16) * 1000

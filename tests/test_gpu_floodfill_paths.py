@@ -1,6 +1,7 @@
-"""Flood-fill paths that the parity tests of test_gpu_floodfill.py do not reach: every tuning knob
-(each in a process of its own), more than 1024 tiles, floods of thousands of rounds and the round
-cap, and int16 and uint8 data and thresholds at their limits through every build of the bit volumes.
+"""Flood-fill paths that the parity tests of test_gpu_floodfill.py do not reach: the tuning knob
+B2V_FF_GRID (each setting in a process of its own), more than 1024 tiles, floods of thousands of
+rounds and the round cap, and int16 and uint8 data and thresholds at their limits through every
+build of the bit volumes.
 
 Every device result is compared bit for bit with the serial C checker; where the element is
 symmetric and the volume large, also with the seeded components of the passable set that
@@ -80,10 +81,10 @@ def _layout_tiles(shape):
 # ---------------------------------------------------------------------------------- A. tuning knobs
 @pytest.mark.parametrize("setting", list(knob.SETTINGS))
 def test_floodfill_knob_setting(orc, tmp_path, setting):
-    """One process per knob setting (the knobs are read once per process): every case of the
+    """One process per knob setting (the knob is read once per process): every case of the
     setting on both engines against the checker, and proof that the setting took effect: the
-    tile count of B2V_FF_TILE=8, and for B2V_FF_GRID the fallback signature (the host-driven rounds
-    ran: the persistent kernel's round counter stayed 0, the returned count did not)."""
+    fallback signature (the host-driven rounds ran: the persistent kernel's round counter stayed 0,
+    the returned count did not)."""
     knobs, shapes = knob.SETTINGS[setting]
     env = {k: v for k, v in os.environ.items() if not k.startswith("B2V_FF_")}
     env.update(knobs)
@@ -93,16 +94,14 @@ def test_floodfill_knob_setting(orc, tmp_path, setting):
     r = subprocess.run(cmd, env=env, timeout=900, capture_output=True, text=True)
     assert r.returncode == 0, f"child failed ({r.returncode}):\n{r.stdout[-4000:]}\n{r.stderr[-8000:]}"
     res = json.loads((tmp_path / "results.json").read_text())
-    edge = knob.tile_edge(setting)
-    grid = int(knobs.get("B2V_FF_GRID", 0))
+    grid = int(knobs["B2V_FF_GRID"])
     for cname, sname, ename in knob.cases(setting):
         shape = shapes[sname]
-        tiles = knob.tile_count(shape, edge)
-        if not any(k.startswith("B2V_FF_") for k in os.environ):
-            assert _layout_tiles(shape) == knob.tile_count(shape, 16), shape    # the restatement is right
-        (tz, ty, tw), _ = knob.tile_shape(shape, edge)
-        assert ((tw, ty, tz) == (16, edge, edge)) == (sname in ("canon", "big")), (shape, tz, ty, tw)
-        fallback = grid > 0 and grid * knob.MAX_MINE < tiles
+        tiles = knob.tile_count(shape)
+        assert _layout_tiles(shape) == tiles, shape    # the restatement is right
+        (tz, ty, tw), _ = knob.tile_shape(shape)
+        assert ((tw, ty, tz) == (16, 16, 16)) == (sname == "canon"), (shape, tz, ty, tw)
+        fallback = grid * knob.MAX_MINE < tiles
         assert fallback == (sname == "fallback"), (setting, sname, tiles)
         c = knob.case_inputs(setting, sname, ename)
         args = (c["data"], c["seeds"], c["t0"], c["t1"], c["fill"], c["strct"], c["out0"])
@@ -116,8 +115,6 @@ def test_floodfill_knob_setting(orc, tmp_path, setting):
             assert np.array_equal(got, want), (key, int((got != want).sum()))
             rec = res[key]
             assert rec["tiles"] == tiles, (key, rec)
-            if edge == 8:
-                assert rec["tiles"] != knob.tile_count(shape, 16), key
             assert rec["rounds"] > 0, (key, rec)
             if engine == "persistent" and not fallback:
                 assert rec["stats_rounds"] == rec["rounds"], (key, rec)
